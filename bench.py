@@ -2,7 +2,7 @@
 """bench.py -- throughput of the BPE-encode hot path (BASELINE.json metric: input GB/s and
 Mtokens/s, cl100k_base, 1 GiB synthetic English-like corpus = SURVEY.md 8(d) config 2).
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload config2]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--workload config2] [--dump-outputs DIR]
 
 A "step" = one pass of the hot path over one batch (the whole workload of this rank).
   value    device-resident: text + doc offsets already in HBM, tokens + offsets left in HBM.  The K steps are
@@ -22,6 +22,11 @@ A "step" = one pass of the hot path over one batch (the whole workload of this r
   cpu_baseline / --impl reference: the reference engine itself (the tiktoken wheel's Rust CoreBPE
            driven through tiktoken.Encoding.encode_ordinary_batch with all host cores) on a bounded
            sample of the same workload; if the wheel cannot be imported, the oracle port.
+  --dump-outputs DIR  after the timed steps, what the last timed step returned (rank 0): DIR/tokens.npy and
+           DIR/token_offsets.npy as float64 (exact: ids < 2^32, offsets < 2^53).  An array longer than its cap is
+           reduced to the positions np.unique(np.random.default_rng(DUMP_SEED + k).integers(0, n, cap)), written next
+           to it as DIR/<name>_index.npy, so that two builds run with the same arguments (same seeded inputs) can be
+           compared output for output, and a difference in length shows in the index.
 N > 1 (torchrun, one rank per GPU): documents shard across ranks (weak scaling: every rank has its
 own corpus of the configured size); the only exchange is an NCCL all-gather of per-rank counts.
 Every rank is gated against the oracle before any number is reported.
@@ -56,6 +61,8 @@ WORKLOADS = {
 }
 DEFAULT_BYTES = {"config1": 1 << 20, "config2": 1 << 30, "config3": 1 << 30, "config4": 1_020_000_000, "config5": 64 << 20}
 SEEDS = {"config1": 1001, "config2": 1002, "config3": 1003, "config4": 1004, "config5": 1005}
+DUMP_SEED = 12345
+DUMP_CAPS = {"tokens": 3 << 20, "token_offsets": 1 << 19}      # float64 entries, values + index: 56 MiB at most
 
 
 def measured_peak():
@@ -65,7 +72,7 @@ def measured_peak():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM HBM3), not measured"
 
 
 class ClockSampler:
@@ -93,8 +100,8 @@ class ClockSampler:
 
     def stop(self, t0=None, t1=None, t_warm=None):
         """Clocks from the samples that arrived inside [t0, t1] (the timed region).  The sampler is started before the
-        warm-up steps so that it is already running; when fewer than three samples fall inside the timed region (five
-        6.7 ms steps are one or two 10 ms sampling periods) the window is widened to the identical warm-up steps that
+        warm-up steps so that it is already running; when fewer than three samples fall inside the timed region (a few
+        steps of a few ms span one or two 10 ms sampling periods) the window is widened to the identical warm-up steps that
         run back to back before it (from t_warm) and the line says so."""
         if not self.proc:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
@@ -270,6 +277,24 @@ class Bench:
         self.torch.cuda.empty_cache()
 
 
+def dump_outputs(b: Bench, n_tok, out_dir):
+    """Write the device-resident result of the last step (tokens, per-document token offsets) as float64 .npy files,
+    each reduced to a fixed seeded sample of positions when longer than its cap (DUMP_CAPS); the sampled positions are
+    written as <name>_index.npy."""
+    torch = b.torch
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"tokens": (b.d_tok, n_tok, np.uint32), "token_offsets": (b.d_toff, b.n_docs + 1, np.int64)}
+    for k, (name, (dev, n, kind)) in enumerate(arrays.items()):
+        cap = DUMP_CAPS[name]
+        if n <= cap:
+            host = dev[:n].cpu().numpy()
+        else:
+            idx = np.unique(np.random.default_rng(DUMP_SEED + k).integers(0, n, cap))
+            host = dev[torch.from_numpy(idx).to(dev.device)].cpu().numpy()
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+        np.save(os.path.join(out_dir, name + ".npy"), host.view(kind).astype(np.float64))
+
+
 def timed_device_loop(b: Bench, steps, world, xchg):
     """K steps enqueued back to back on b.stream, one NCCL count exchange per step enqueued behind each pipeline;
     CUDA events on that stream; returns ms for the K steps (this rank)."""
@@ -302,6 +327,8 @@ def main():
     ap.add_argument("--no-configs", action="store_true", help="skip the block with the other BASELINE configs")
     ap.add_argument("--no-extras", action="store_true", help="skip api / strong-scaling / one-process multi-GPU lines")
     ap.add_argument("--decode", action="store_true", help="also time the device decode of the produced tokens (next row)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float64, seeded sample when large)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
 
@@ -315,7 +342,7 @@ def main():
     def config_of(workload, nb, parallelism=None):
         e, _, d = WORKLOADS[workload]
         return {"workload": f"{workload}: {d}", "bytes_per_gpu": nb, "encoding": e, "seed": SEEDS[workload],
-                "l2": "inputs (>= 64 MiB text per step, streamed once) exceed or equal the 126 MB L2; no reuse between steps",
+                "l2": "inputs (>= 64 MiB text per step, streamed once) exceed the 50 MB L2; no reuse between steps",
                 "parallelism": parallelism or f"doc-sharded x{world}"}
 
     # ---------------------------------------------------------------- reference arm (CPU)
@@ -344,7 +371,7 @@ def main():
         print(json.dumps(line))
         return 0
 
-    # ---------------------------------------------------------------- B200 arm
+    # ---------------------------------------------------------------- GPU arm
     import torch
     import torch.distributed as dist
     if not torch.cuda.is_available():
@@ -396,7 +423,7 @@ def main():
             dist.all_reduce(t, op=dist.ReduceOp.SUM)
         return int(t.item()) == 0
 
-    def measure(b: Bench, steps, warmup, sample_clocks=False):
+    def measure(b: Bench, steps, warmup, sample_clocks=False, dump_dir=None):
         """parity gate (every rank) -> value -> e2e (compared with the device result); returns a dict."""
         ok, n_tok = b.parity(cores)
         if not allok(ok):
@@ -420,6 +447,8 @@ def main():
         t1 = time.perf_counter()
         barrier()
         clocks = sampler.stop(t0, t1, t_warm) if sampler else None
+        if dump_dir and rank == 0:
+            dump_outputs(b, n_tok, dump_dir)
         per_rank = [ms_total / steps]
         if world > 1:                                           # which rank set the pace (the MAX is what counts)
             t = torch.tensor([ms_total / steps], dtype=torch.float64, device="cuda")
@@ -444,7 +473,7 @@ def main():
                 "clocks": clocks, "counts_exchanged": [int(x) for x in placements[-1][0][:, 0]] if placements else None}
 
     b = Bench(args.workload, nbytes, rank, world, local_rank, seed_offset=7919 * rank)   # weak scaling: own corpus per rank
-    m = measure(b, args.steps, args.warmup, sample_clocks=True)
+    m = measure(b, args.steps, args.warmup, sample_clocks=True, dump_dir=args.dump_outputs)
     if not m.get("parity"):
         if rank == 0:
             print(json.dumps({"error": m.get("error", "e2e result differs from the device-resident result"), "detail": m}))
@@ -466,13 +495,6 @@ def main():
            "long-piece kernels": None}
     dominant = max((k for k in kern_ms if alg[k]), key=lambda k: kern_ms[k])
     achieved = alg[dominant] / (kern_ms[dominant] * 1e-3) / 1e9
-    traffic = None
-    prof = os.path.join(ROOT, "profiles", "ncu_traffic.json")
-    if os.path.exists(prof):
-        try:
-            traffic = json.load(open(prof)).get(dominant.split("+")[-1], {}).get("dram_bytes_per_launch")
-        except Exception:
-            traffic = None
     pipeline_alg = N + 4 * n_tok + 16 * (n_docs + 1)                    # SURVEY 8(d): text + tokens + both offset arrays
     dev_ms = stage["device_total_ms"]
     line = {
@@ -486,7 +508,7 @@ def main():
         "per_rank_ms_per_step": m["per_rank_ms_per_step"],
         "stage_ms": stage, "kernel_ms": kern_ms,
         "roofline": {"bound": "hbm", "kernel": dominant, "achieved": achieved, "peak": peak, "unit": "GB/s",
-                     "frac": achieved / peak, "traffic": traffic, "peak_source": peak_src,
+                     "frac": achieved / peak, "peak_source": peak_src,
                      "algorithmic_bytes_per_launch": alg[dominant], "kernel_ms": kern_ms[dominant],
                      "per_kernel": {k: {"ms": kern_ms[k], "algorithmic_bytes": alg[k],
                                         "frac": (alg[k] / (kern_ms[k] * 1e-3) / 1e9 / peak) if alg[k] and kern_ms[k] > 0 else None}
@@ -596,7 +618,7 @@ def main():
                 nb = DEFAULT_BYTES[w]
                 single = w in ("config5", "config1")                 # one document: does not shard -> replicas (DESIGN 5)
                 bw = Bench(w, nb, rank, world, local_rank, seed_offset=0 if single else 7919 * rank)
-                mw = measure(bw, 3, 2)
+                mw = measure(bw, args.steps, args.warmup)
                 entry = {"config": config_of(w, nb, "replicas (one document cannot shard)" if single else None)}
                 entry["config"]["vocab"] = f"{bw.vocab_src} ({len(bw.ranks)} mergeable ranks)"
                 entry.update({k: mw.get(k) for k in ("parity", "value", "ms_per_step", "mtokens_per_s", "stage_ms", "error")})

@@ -1,5 +1,5 @@
 /*
- * b200bpe.h -- C ABI of libb200bpe.so, the B200-native BPE encoder that replaces tiktoken's
+ * b200bpe.h -- C ABI of libb200bpe.so, the H100-native BPE encoder that replaces tiktoken's
  * Rust extension `_tiktoken` (reference: openai/tiktoken v0.14.0, src/lib.rs + src/py.rs).
  *
  * Boundary: this is exactly what a `_tiktoken` replacement binds.  Each entry point names the
@@ -7,7 +7,7 @@
  * sizes only; no torch / Python types.  All functions return 0 on success and a negative
  * B200BPE_E* code on failure; `b200bpe_last_error()` returns a thread-local message.
  *
- * There is no CPU fallback: every encode call runs the sm_100a kernels on the device the
+ * There is no CPU fallback: every encode call runs the sm_90a kernels on the device the
  * engine was created on, and fails with B200BPE_ECUDA if that is not possible.
  */
 #ifndef B200BPE_H

@@ -25,7 +25,7 @@ def test_library_builds_and_exports_every_declared_symbol():
     for s in syms:
         assert hasattr(L, s), f"{s} declared in include/b200bpe.h but not exported"
     assert sorted(_lib.EXPORTS) == syms
-    assert b"sm_100a" in _lib.lib().b200bpe_version()
+    assert b"sm_90a" in _lib.lib().b200bpe_version()
 
 
 def test_unsupported_pattern_is_value_error():

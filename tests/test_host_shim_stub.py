@@ -249,7 +249,7 @@ def test_pickle_by_value_rebuilds_the_engine(enc):
 def test_registry_is_the_references_and_pickles_by_reference(enc, monkeypatch):
     """`tiktoken_b200.get_encoding` serves the constructors the reference's own registry discovers among the
     `tiktoken_ext` plugins (tiktoken/registry.py) -- here one more entry, as a plugin would publish it -- builds the
-    B200-backed class once per name and pickles it by name (tiktoken/core.py:409-417)."""
+    GPU-backed class once per name and pickles it by name (tiktoken/core.py:409-417)."""
     import tiktoken.registry as ref_registry
     import tiktoken_b200
     pat, ranks, special, _ = vu.load_encoding("r50k_base", allow_real=False)

@@ -213,11 +213,10 @@ def test_malformed_utf8_terminates(hostcheck):
 
 
 def test_cl100k_contraction_rule_is_exact(hostcheck):
-    """The cl100k contraction rule (landed in round 2 after the GPU A/B, profiles/r02_c_pretok_flag_ab.txt: pretok
-    1.99 -> 1.71 ms per GiB of English): letters 2..3 bytes after an apostrophe decided per apostrophe (is it
+    """The cl100k contraction rule: letters 2..3 bytes after an apostrophe decided per apostrophe (is it
     's|'t|'re|'ve|'m|'ll|'d, where does it end) instead of by the general function; with it English text has no
-    undecided position left.  The whitespace-after-CR/LF cases stay with the general function (a bit-parallel rule for
-    them was measured without gain and dropped) and are checked here all the same."""
+    undecided position left.  The whitespace-after-CR/LF cases stay with the general function (there is no bit-parallel
+    rule for them) and are checked here all the same."""
     H = hostcheck
     pid, pat = PATS["cl100k"]
     o = Oracle(BYTES, {}, pat)
@@ -271,8 +270,7 @@ def test_cl100k_contraction_rule_is_exact(hostcheck):
 
 
 def test_r50k_contractions_at_every_alignment(hostcheck):
-    """The case-sensitive `'(?:[sdmt]|ll|ve|re)` of the r50k / p50k pattern (decided by the general function: a
-    per-apostrophe fast rule was measured without gain on the GPU and dropped).  Documents are packed back to back,
+    """The case-sensitive `'(?:[sdmt]|ll|ve|re)` of the r50k / p50k pattern (decided by the general function).  Documents are packed back to back,
     so apostrophes also meet across document boundaries."""
     H = hostcheck
     pid, pat = PATS["r50k"]
@@ -302,8 +300,7 @@ def test_r50k_contractions_at_every_alignment(hostcheck):
 
 
 def test_o200k_prefix_and_apostrophe_rules_are_exact(hostcheck):
-    """The two o200k rules landed in round 2 after the GPU A/B (profiles/r02_c_pretok_flag_ab.txt: pretok 4.71 -> 3.31
-    ms per 256 MiB of mixed-script text): a letter after a punctuation scalar decided bit-parallel as
+    """The two o200k rules: a letter after a punctuation scalar decided bit-parallel as
     boundary(p) = !boundary(x), and apostrophes / contraction tails decided per apostrophe.  Exhaustive strings, the
     real engine's random Unicode splits, a mixed-script corpus, and a short fuzz run."""
     import subprocess

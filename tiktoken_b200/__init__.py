@@ -1,11 +1,11 @@
-"""tiktoken_b200 -- B200-native BPE encoder behind tiktoken's API (encode hot path only).
+"""tiktoken_b200 -- H100-native BPE encoder behind tiktoken's API (encode hot path only).
 
     from tiktoken_b200 import Encoding          # tiktoken.Encoding's constructor (+ device= / devices=)
     enc = Encoding("my_enc", pat_str=..., mergeable_ranks=..., special_tokens=...)
-    enc.encode_ordinary_batch(docs)             # one native call -> sm_100a kernels
+    enc.encode_ordinary_batch(docs)             # one native call -> sm_90a kernels
 
-    tiktoken_b200.get_encoding("cl100k_base")   # the reference's registry + plugins, B200-backed Encoding
-    tiktoken_b200.install()                     # or: run the UNMODIFIED `tiktoken` package on the B200 engine
+    tiktoken_b200.get_encoding("cl100k_base")   # the reference's registry + plugins, GPU-backed Encoding
+    tiktoken_b200.install()                     # or: run the UNMODIFIED `tiktoken` package on the GPU engine
 
 `tiktoken_b200._tiktoken.CoreBPE` is the drop-in for the Rust extension (see INTEGRATION.md).  Everything the
 north star says stays -- tiktoken/core.py's host class, tiktoken/registry.py, tiktoken/load.py, the tiktoken_ext
@@ -33,7 +33,7 @@ def _constructors():
 
 
 def get_encoding(encoding_name: str, **device_kw) -> Encoding:
-    """`tiktoken.get_encoding` with the B200-backed class: same names, same plugin constructors
+    """`tiktoken.get_encoding` with the GPU-backed class: same names, same plugin constructors
     (tiktoken_ext.openai_public, ...), one cached instance per name."""
     if not isinstance(encoding_name, str):
         raise ValueError(f"Expected a string in get_encoding, got {type(encoding_name)}")
@@ -53,7 +53,7 @@ def list_encoding_names() -> list[str]:
 
 
 def install() -> None:
-    """Make the unmodified `tiktoken` package use the B200 engine from now on: `tiktoken.core._tiktoken` (the one
+    """Make the unmodified `tiktoken` package use the GPU engine from now on: `tiktoken.core._tiktoken` (the one
     name through which tiktoken/core.py reaches its native module, core.py:7,54) becomes `tiktoken_b200._tiktoken`.
     Every `tiktoken.Encoding` constructed afterwards -- `tiktoken.get_encoding(...)` included -- runs on the GPU.
     This is what shipping `tiktoken/_tiktoken.py` = this shim in place of the Rust extension does (INTEGRATION.md)."""

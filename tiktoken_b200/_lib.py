@@ -3,7 +3,7 @@
 This is the binding a tiktoken maintainer would add in place of the PyO3 module
 (src/py.rs): plain pointers and sizes, the GIL is released for the duration of every call
 (ctypes.CDLL does that), errors come back as status codes + a thread-local message.
-The library is built in-tree by `build()` (nvcc, sm_100a only).  There is no fallback: if the
+The library is built in-tree by `build()` (nvcc, sm_90a only).  There is no fallback: if the
 shared object or a CUDA device is missing the import / constructor raises.
 """
 from __future__ import annotations
@@ -20,12 +20,12 @@ _SOURCES = ["b200bpe.cu", "dev_common.cuh", "kernels_pretok.cuh", "kernels_long.
 
 OK, EINVAL, EPATTERN, EDUPRANK, ECUDA, ENOBYTE, EKEY, ESPECIAL, ECAPACITY = 0, -1, -2, -3, -4, -5, -6, -7, -8
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
 
 
 def build(force: bool = False) -> str:
-    """Compile libb200bpe.so for sm_100a with nvcc (cross-compiles without a GPU)."""
+    """Compile libb200bpe.so for sm_90a with nvcc (cross-compiles without a GPU)."""
     srcs = [os.path.join(_CSRC, s) for s in _SOURCES] + [
         os.path.join(os.path.dirname(_CSRC), "..", "include", "b200bpe.h")]
     stale = force or not os.path.exists(_SO) or any(

@@ -3,7 +3,7 @@
 `CoreBPE(mergeable_ranks, special_tokens, pat_str)` has the constructor and the methods
 `tiktoken/core.py` calls on `self._core_bpe` (core.py:57,76,127,161,259,273,301,358,393),
 plus two batched entry points (`encode_ordinary_batch`, `encode_batch`) that the host class
-uses instead of a thread pool: one native call per batch, executed by hand-written sm_100a
+uses instead of a thread pool: one native call per batch, executed by hand-written sm_90a
 kernels through the C ABI of libb200bpe.so.  No CPU fallback exists.
 """
 from __future__ import annotations
@@ -272,7 +272,7 @@ class CoreBPE:
         except UnicodeDecodeError:
             raise NotImplementedError(
                 "_encode_bytes on invalid UTF-8 (unstable-token path, src/py.rs:79-112) is out of scope "
-                "of the B200 encoder") from None
+                "of the GPU encoder") from None
         return self.encode_ordinary(text)
 
     def encode_with_unstable(self, text: str, allowed_special):             # py.rs:117-131

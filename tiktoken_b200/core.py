@@ -1,16 +1,16 @@
 """`tiktoken_b200.Encoding` -- the reference's own host class (`tiktoken.core.Encoding`, which STAYS: special-token
-policy, surrogate fix-up, decode helpers, pickling, ...) running on the B200 engine, with the batch methods
+policy, surrogate fix-up, decode helpers, pickling, ...) running on the GPU engine, with the batch methods
 replaced by ONE native call per batch.
 
 What this file adds to the inherited class, and nothing else:
-  * the constructor builds `tiktoken_b200._tiktoken.CoreBPE` (ctypes -> libb200bpe.so -> sm_100a kernels) where
+  * the constructor builds `tiktoken_b200._tiktoken.CoreBPE` (ctypes -> libb200bpe.so -> sm_90a kernels) where
     the reference builds the Rust extension's (tiktoken/core.py:54-57), optionally on several GPUs (`devices=`);
   * `encode_ordinary_batch` / `encode_batch` / `decode_batch` / `decode_bytes_batch` make one native call for the
     whole batch instead of a ThreadPoolExecutor over per-document calls (core.py:161-203, :334-350); `num_threads`
     is accepted and ignored (the GPU is the pool); the disallowed-special check of `encode_batch` runs inside the same
     device scan that cuts the documents at allowed specials, instead of a Python regex search per document;
   * array-returning variants (`*_to_numpy`, `*_packed`) that never build Python lists.
-For a process that should run the UNMODIFIED reference package on the B200 engine, see `tiktoken_b200.install()`.
+For a process that should run the UNMODIFIED reference package on the GPU engine, see `tiktoken_b200.install()`.
 """
 from __future__ import annotations
 

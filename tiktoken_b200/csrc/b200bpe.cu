@@ -1,4 +1,4 @@
-// b200bpe.cu -- the engine and the C ABI of libb200bpe.so (see include/b200bpe.h).  sm_100a only.
+// b200bpe.cu -- the engine and the C ABI of libb200bpe.so (see include/b200bpe.h).  sm_90a only.
 //
 // Path replaced: CoreBPE::encode_ordinary / CoreBPE::encode (src/lib.rs:360-442) and the per-call
 // thread pool that fans documents out to it (tiktoken/core.py:164-206).  One call encodes the
@@ -250,6 +250,7 @@ struct DevCtx {
     static const int N_SLOTS = B2_N_SLOTS;
     Slot slots[B2_N_SLOTS];
     size_t l2_window = 0; float l2_ratio = 0.f;
+    int n_sm = 0;                     // multiprocessors: the persistent and work-queue kernels launch a multiple of this
     int probe_blocks_per_sm = 10;
 };
 
@@ -317,7 +318,7 @@ struct b200bpe {
 };
 
 extern "C" const char *b200bpe_last_error(void) { return g_last_error.c_str(); }
-extern "C" const char *b200bpe_version(void) { return "b200bpe 0.2 (sm_100a)"; }
+extern "C" const char *b200bpe_version(void) { return "b200bpe 0.2 (sm_90a)"; }
 extern "C" int b200bpe_device_count(void) {
     int n = 0;
     if (cudaGetDeviceCount(&n) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -356,6 +357,7 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
     D->device = device;
     const HostTables &H = h->H;
     cudaError_t e = cudaSetDevice(device);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&D->n_sm, cudaDevAttrMultiProcessorCount, device);
     uint8_t ascii[128];
     for (int i = 0; i < 128; i++) ascii[i] = UC_STAGE2[(uint32_t)UC_STAGE1[0] * 256 + i];
     // one arena, hottest tables first: the L2 persistence window covers a prefix of it
@@ -395,10 +397,10 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
     D->T.long_tab = (const U4 *)(D->arena + parts[7].off); D->T.long_mask = H.long_mask;
     D->T.long_blob = D->arena + parts[8].off;
     D->T.max_token_len = H.max_token_len; D->T.n_long_tokens = H.n_long_tokens;
-    // L2 persistence (off by default): a persisting access-policy window over the rank tables was measured on B200 at
-    // 1 GiB of English text -- probe_kernel 2.78 ms with the window vs 2.60 ms without, whole step 8.64 vs 8.43 ms
-    // (profiles/r02_b_knobs.txt): the tables already stay in the 126 MB L2 (they are re-touched every few microseconds)
-    // and the set-aside only shrinks what the streams can use.  B200BPE_L2_PERSIST=1 turns it on for experiments.
+    // L2 persistence (off by default): a persisting access-policy window over the rank tables was measured on an H100
+    // 80GB HBM3 (SXM, 700 W power limit) at 1 GiB per step -- cl100k English 120.8 GB/s without the window vs 64.6 with
+    // it, o200k mixed scripts 23.9 vs 19.2: the set-aside costs the streams far more than it saves the table probes.
+    // B200BPE_L2_PERSIST=1 turns it on for experiments.
     if (env_long("B200BPE_L2_PERSIST", 0, 0, 1)) {
         int max_win = 0, max_persist = 0;
         cudaDeviceGetAttribute(&max_win, cudaDevAttrMaxAccessPolicyWindowSize, device);
@@ -427,7 +429,7 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
     else if (strcmp(pat_str, CL100K_PAT) == 0) pattern = PAT_CL100K;
     else if (strcmp(pat_str, O200K_PAT) == 0) pattern = PAT_O200K;
     else return fail(B200BPE_EPATTERN,
-                     "unsupported pat_str: the B200 pre-tokeniser implements exactly the r50k/p50k, cl100k and "
+                     "unsupported pat_str: the GPU pre-tokeniser implements exactly the r50k/p50k, cl100k and "
                      "o200k patterns of tiktoken_ext/openai_public.py (there is no CPU regex fallback)");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
@@ -486,7 +488,7 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
         int bits = 1;
         while (bits < 32 && (max_id >> bits)) bits++;
         bits = std::max(bits, 8);
-        h->pack_bits = (bits <= 24 && env_long("B200BPE_PACK", 0, 0, 1)) ? bits : 0;   // opt-in: see DESIGN 4 (measured: no gain)
+        h->pack_bits = (bits <= 24 && env_long("B200BPE_PACK", 0, 0, 1)) ? bits : 0;   // opt-in: see DESIGN 4
     }
     h->table_bytes[0] = H.piece_tab.size() * sizeof(U4);
     h->table_bytes[1] = H.pair_tab.size() * sizeof(U4) + 65536 * 4 + 1024;
@@ -586,7 +588,7 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         CUDA_TRY(S.w_mq_len.ensure(mcap));
         CUDA_TRY(S.w_mq_key.ensure(mcap)); CUDA_TRY(S.w_mq_skey.ensure(mcap)); CUDA_TRY(S.w_mq_smeta.ensure(mcap));
         CUDA_TRY(S.w_mres.ensure(S.mres_cap + 64));
-        CUDA_TRY(S.w_sort_hist.ensure((size_t)SORT_BLOCKS * 17 + 32));
+        CUDA_TRY(S.w_sort_hist.ensure((size_t)D->n_sm * SORT_BLOCKS_PER_SM * 17 + 32));
     }
     {   // undecided pre-tokeniser positions: under 2 % on the worst corpus seen; sized for 12 %, grown on ERR_SLOWCAP
         const size_t want = std::max<size_t>((size_t)(n_bytes / 8) + 4096, MISS_CAP_MIN);
@@ -663,7 +665,7 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
 #define B2_PRETOK(P)                                                                                                                   \
     pretok_kernel<P><<<grid, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, n_words, ibits,          \
                                           S.w_slow.p, scap, S.d_ctr);                                                                  \
-    pretok_slow_kernel<P><<<148 * 8, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, S.w_slow.p, scap, S.d_ctr)
+    pretok_slow_kernel<P><<<D->n_sm * 8, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, S.w_slow.p, scap, S.d_ctr)
             if (h->pattern == PAT_R50K) { B2_PRETOK(PAT_R50K); }
             else if (h->pattern == PAT_CL100K) { B2_PRETOK(PAT_CL100K); }
             else { B2_PRETOK(PAT_O200K); }
@@ -686,22 +688,22 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         CUDA_TRY(cudaEventRecord(S.ev[11], ls));
         LongScratch LS{S.w_idA.p, S.w_rkA.p, S.w_idB.p, S.w_rkB.p, S.w_aux1.p, S.w_aux2.p, S.w_flag.p};
         if (h->pmerge) {         // 129..1024 bytes: segmented parallel merge (rounds, not merges, are sequential); shorter: a group of lanes per piece
-            pmerge_kernel<256, 3><<<148 * 10, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            pmerge_long_kernel<<<148 * 4, PM_WARPS_L * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            if (h->pmerge_min_cls <= 2) pmerge_kernel<128, 2><<<148 * 16, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            else mid_group32_kernel<<<148 * 4, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 2);
-            if (h->pmerge_min_cls <= 1) pmerge_kernel<64, 1><<<148 * 16, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            mid_group16_kernel<<<148 * 9, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, h->pmerge_min_cls <= 1 ? 0 : 1);
+            pmerge_kernel<256, 3><<<D->n_sm * 10, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
+            pmerge_long_kernel<<<D->n_sm * 4, PM_WARPS_L * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
+            if (h->pmerge_min_cls <= 2) pmerge_kernel<128, 2><<<D->n_sm * 16, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
+            else mid_group32_kernel<<<D->n_sm * 4, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 2);
+            if (h->pmerge_min_cls <= 1) pmerge_kernel<64, 1><<<D->n_sm * 16, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
+            mid_group16_kernel<<<D->n_sm * 9, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, h->pmerge_min_cls <= 1 ? 0 : 1);
         } else if (h->mid_group) {      // 17..1024 bytes: a group of lanes per piece, state in shared memory
-            mid_group32_kernel<<<148 * 4, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 4);
-            mid_group16_kernel<<<148 * 9, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 1);
+            mid_group32_kernel<<<D->n_sm * 4, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 4);
+            mid_group16_kernel<<<D->n_sm * 9, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 1);
         } else {                 // ranks of 2^22 and above: one piece per lane (72 KiB of columns per block) / warp per piece
-            mid_thread_kernel<<<148 * 3, MID_WARPS * 32, MID_SMEM_BYTES, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            long_piece_kernel<<<148 * 8, LONG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr, CLS_G1024);
+            mid_thread_kernel<<<D->n_sm * 3, MID_WARPS * 32, MID_SMEM_BYTES, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
+            long_piece_kernel<<<D->n_sm * 8, LONG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr, CLS_G1024);
         }
-        long_piece_kernel<<<148 * 8, LONG_WARPS * 32, 0, ls2>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr, CLS_WARP);
-        giant_piece_kernel<<<148, GIANT_THREADS, 0, ls2>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr);
-        cluster_piece_kernel<<<(148 / CLUSTER_CTAS) * CLUSTER_CTAS, GIANT_THREADS, 0, ls2>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr);
+        long_piece_kernel<<<D->n_sm * 8, LONG_WARPS * 32, 0, ls2>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr, CLS_WARP);
+        giant_piece_kernel<<<D->n_sm, GIANT_THREADS, 0, ls2>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr);
+        cluster_piece_kernel<<<(D->n_sm / CLUSTER_CTAS) * CLUSTER_CTAS, GIANT_THREADS, 0, ls2>>>(a.d_text, D->T, q, LS, S.w_ltok.p, S.d_ctr);
         CUDA_TRY(cudaEventRecord(S.ev[13], ls2));
         CUDA_TRY(cudaEventRecord(S.ev[12], ls));
         launches += 5;
@@ -721,13 +723,14 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         p.out = a.d_out; p.tok_off = a.d_tok_off; p.ctr = S.d_ctr;
         p.big_dst = S.w_big_dst.p; p.big_src = S.w_big_src.p; p.big_n = S.w_big_n.p;
         const long long want_blocks = (n_tiles + ENC_WARPS - 1) / ENC_WARPS;
-        const unsigned probe_grid = (unsigned)std::min<long long>(want_blocks, 148ll * D->probe_blocks_per_sm);
+        const unsigned probe_grid = (unsigned)std::min<long long>(want_blocks, (long long)D->n_sm * D->probe_blocks_per_sm);
         probe_kernel<<<probe_grid, ENC_WARPS * 32, 0, st>>>(p, D->T);
         CUDA_TRY(cudaEventRecord(S.ev[8], st));
-        miss_hist_kernel<<<SORT_BLOCKS, 256, 0, st>>>(p, S.w_sort_hist.p);
-        miss_base_kernel<<<1, 17 * 32, 0, st>>>(S.w_sort_hist.p, SORT_BLOCKS);
-        miss_scatter_kernel<<<SORT_BLOCKS, 256, 0, st>>>(p, S.w_sort_hist.p);
-        miss_kernel<<<148 * 16, MISS_WARPS * 32, 0, st>>>(p, D->T);
+        const int sort_blocks = D->n_sm * SORT_BLOCKS_PER_SM;
+        miss_hist_kernel<<<sort_blocks, 256, 0, st>>>(p, S.w_sort_hist.p);
+        miss_base_kernel<<<1, 17 * 32, 0, st>>>(S.w_sort_hist.p, sort_blocks);
+        miss_scatter_kernel<<<sort_blocks, 256, 0, st>>>(p, S.w_sort_hist.p);
+        miss_kernel<<<D->n_sm * 16, MISS_WARPS * 32, 0, st>>>(p, D->T);
         CUDA_TRY(cudaEventRecord(S.ev[7], st));
         CUDA_TRY(cudaStreamWaitEvent(st, S.ev[12], 0));          // join: the long pieces' tokens and counts are needed from here on
         CUDA_TRY(cudaStreamWaitEvent(st, S.ev[13], 0));
@@ -742,7 +745,7 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
             gather_kernel<0><<<gather_grid, GATHER_WARPS * 32, 0, st>>>(p);
             gather_kernel<1><<<(unsigned)((n_docs + 1 + GATHER_WARPS - 1) / GATHER_WARPS), GATHER_WARPS * 32, 0, st>>>(p);
         } else gather_kernel<2><<<gather_grid, GATHER_WARPS * 32, 0, st>>>(p);
-        big_copy_kernel<<<148 * 2, 256, 0, st>>>(p);
+        big_copy_kernel<<<D->n_sm * 2, 256, 0, st>>>(p);
         finalize_kernel<<<1, 32, 0, st>>>(S.d_ctr, S.d_sticky, a.d_counts, n_docs);
         launches += sparse_docs ? 12 : 11;
     }
@@ -955,10 +958,9 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     auto slot_of = [&](size_t k) -> Slot & { return D->slots[k % DevCtx::N_SLOTS]; };
 
     // Upload of chunk k into its slot.  Pinned caller memory: on the slot's own stream, i.e. behind the download of the
-    // slot's previous chunk -- measured better than letting uploads run free (free-running uploads and downloads fight for
-    // the link: 38.8 vs 41.4 GB/s end to end).  Pageable caller memory: helper threads fill a pinned block quarter by
-    // quarter and the quarters go up on the slot's UPLOAD stream, which only waits for the kernels (ev[4]) of the slot's
-    // previous chunk, so that the host never sits behind a download (18 -> 22 GB/s).
+    // slot's previous chunk, so that uploads and downloads do not run free and fight for the link.  Pageable caller
+    // memory: helper threads fill a pinned block quarter by quarter and the quarters go up on the slot's UPLOAD stream,
+    // which only waits for the kernels (ev[4]) of the slot's previous chunk, so that the host never sits behind a download.
     auto enqueue_h2d = [&](size_t k) -> int {
         Slot &S = slot_of(k);
         const size_t c = mine[k];

@@ -5,7 +5,7 @@
 // of src/lib.rs:140-211 (`_byte_pair_merge`, `byte_pair_encode`) and the whole-piece probe of
 // src/lib.rs:367-368.
 //
-// Design (B200-first, see DESIGN.md):
+// Design (see DESIGN.md):
 //  * token id == rank.  A single byte the vocabulary lacks gets a pseudo id PSEUDO_BASE+byte so
 //    that merges through it still work; emitting one is the reference's panic (lib.rs:202,207).
 //  * PIECE table: open-addressed, 32-byte slots keyed by the piece bytes themselves
@@ -50,11 +50,11 @@ __device__ __forceinline__ U4 ldg_u4(const U4 *p) {
     uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
     U4 r; r.x = v.x; r.y = v.y; r.z = v.z; r.w = v.w; return r;
 }
-// both 16-byte halves of a 32-byte table slot / bucket with ONE 256-bit load (sm_100: LDG.E.256).  The probe and merge
-// kernels are bound by L1TEX wavefronts (ncu: l1tex throughput 80-88 %): a lane-divergent load costs one wavefront per
-// lane whatever its width, so one 32-byte load per probe instead of two 16-byte ones halves the global part.
+// both 16-byte halves of a 32-byte table slot / bucket (one 32-byte sector).  sm_90 has no 256-bit load, so these are
+// two 128-bit loads issued back to back, both in flight before either result is used.
 __device__ __forceinline__ void ldg_u4x2(const U4 *p, U4 &a, U4 &b) {
-    asm("ld.global.nc.v8.u32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
+    asm("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
+        "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
         : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
 }
 #define B2_LDG_U4X2(p, a, b) b2bpe::ldg_u4x2(p, a, b)
@@ -139,7 +139,7 @@ B2_HD void pair_lookup2(const DevTables &T, uint32_t a1, uint32_t b1, uint32_t a
 B2_HD uint32_t piece_lookup16(const DevTables &T, uint64_t k0, uint64_t k1, uint32_t len) {
     uint32_t s = (uint32_t)piece_hash(k0, k1, len) & T.piece_mask;
     for (;;) {
-        U4 k, m; B2_LDG_U4X2(T.piece_tab + 2 * s, k, m);          // both halves of the 32-byte slot: one sector, one load
+        U4 k, m; B2_LDG_U4X2(T.piece_tab + 2 * s, k, m);          // both halves of the 32-byte slot: one sector
         if (m.x == 0) return RANK_MAX;
         if (m.x == len && k.x == (uint32_t)k0 && k.y == (uint32_t)(k0 >> 32) && k.z == (uint32_t)k1 &&
             k.w == (uint32_t)(k1 >> 32))

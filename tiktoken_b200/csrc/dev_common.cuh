@@ -1,4 +1,4 @@
-// dev_common.cuh -- parameter blocks, counters and sm_100a PTX helpers shared by the kernels of libb200bpe.
+// dev_common.cuh -- parameter blocks, counters and sm_90a PTX helpers shared by the kernels of libb200bpe.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -241,11 +241,11 @@ struct MissSmem {
 // counting sort of the miss queue by piece length (so that a warp merges pieces of one length):
 // per-block histograms -> bucket bases -> scatter.  Only block-local shared-memory atomics and
 // 17 values per block in global memory; no hot global counters.
-static const int SORT_BLOCKS = 148 * 2;
+static const int SORT_BLOCKS_PER_SM = 2;
 
 __device__ __forceinline__ uint32_t miss_count(const TileParams &p) { return min(p.ctr->n_miss, p.mq.cap); }
 
-__global__ void __launch_bounds__(256) miss_hist_kernel(TileParams p, unsigned int *block_hist /* [SORT_BLOCKS][17] */) {
+__global__ void __launch_bounds__(256) miss_hist_kernel(TileParams p, unsigned int *block_hist /* [gridDim.x][17] */) {
     __shared__ unsigned int s_h[17];
     if (threadIdx.x < 17) s_h[threadIdx.x] = 0;
     __syncthreads();

@@ -2,7 +2,7 @@
 // GROUP OF LANES per piece.  The literal loop of `_byte_pair_merge` (src/lib.rs:140-196): take the smallest rank
 // (strict `<` => leftmost on ties), merge, re-rank the two neighbouring pairs -- one merge per round.
 //
-// What bounds this stage is the number of warp instructions per merge round (ncu: 88 % issue-active), so the layout is
+// The cost of this stage is the number of warp instructions per merge round, so the layout is
 // chosen to (a) share one instruction stream between as many pieces as possible and (b) keep a round short:
 //   * a piece of up to G*E bytes is spread over G lanes, E parts per lane (G x E = 2x16, 4x16, 4x32, 8x32, 32x32 for
 //     the classes 17-32, 33-64, 65-128, 129-256, 257-1024 bytes): 32 / G pieces walk one convergent instruction stream;

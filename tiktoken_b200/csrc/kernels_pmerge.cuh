@@ -266,9 +266,9 @@ __device__ void pmerge_class(const uint8_t *__restrict__ text, const DevTables &
 }
 
 // One piece per buffer of CAP parts, CAP = the upper length of the class: 129..256 bytes -> 256 parts (4.9 KiB of shared
-// memory per warp, 40 warps per SM), 65..128 -> 128, 33..64 -> 64.  One piece per 256-part buffer beats two per 512-part
-// buffer (9.7 KiB, 20 warps per SM): the kernel is bound by latency and L1TEX, not by instruction issue (config 3, 256 MiB:
-// long-piece stage 7.69 -> 6.92 ms).
+// memory per warp, 40 warps per SM), 65..128 -> 128, 33..64 -> 64.  One piece per 256-part buffer rather than two per
+// 512-part buffer (9.7 KiB, 20 warps per SM): the kernel is meant to hide latency and L1TEX waits with more warps, and
+// instruction issue is not what it spends.
 template <int CAP, int CLS>
 __global__ void __launch_bounds__(PM_WARPS * 32) pmerge_kernel(const uint8_t *__restrict__ text, DevTables T, LongQ q, uint32_t *ltok,
                                                               Counters *ctr) {

@@ -41,7 +41,7 @@ __global__ void mark_docs_kernel(const unsigned long long *__restrict__ doc_off,
 static const int PRETOK_WARPS = 8;
 
 // o200k's rule function is long (case / mark chains): one out-of-line copy serves both call sites; the
-// two shorter ones are cheaper inlined (measured both ways per pattern).
+// two shorter ones are inlined.
 __device__ __noinline__ bool slow_boundary_o200k(const TextAccess &t, long long pos) { return boundary_before<PAT_O200K>(t, pos); }
 
 template <int PAT>
@@ -50,8 +50,8 @@ __device__ __forceinline__ bool slow_boundary(const TextAccess &t, long long pos
     return boundary_before<PAT>(t, pos);
 }
 
-// Fast part: the bit-parallel rules decide all but a fraction of a percent of the positions (none on English text
-// since round 2); the rest go to a global list.  Keeping the general rule function OUT of this kernel keeps its register
+// Fast part: the bit-parallel rules decide all but a fraction of a percent of the positions (none on English text);
+// the rest go to a global list.  Keeping the general rule function OUT of this kernel keeps its register
 // count low and its warps convergent -- the function is long, branchy and walks along runs.
 template <int PAT>
 __global__ void __launch_bounds__(PRETOK_WARPS * 32, PAT == PAT_O200K ? 4 : 5) pretok_kernel(const uint8_t *__restrict__ text, long long n_bytes,

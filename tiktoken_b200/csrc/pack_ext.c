@@ -18,8 +18,7 @@
  * the GIL, the workers only READ those immutable buffers (no Python API off the calling thread; the list keeps the
  * strings alive, the caller waits).  ASCII strings are a memcpy.  str.encode semantics: a lone surrogate raises
  * UnicodeEncodeError (raised by CPython's own encoder on that item, so the exception is the canonical one).
- * (Round 1 went through PyUnicode_AsUTF8AndSize -- CPython's one-thread encoder plus a cached copy per string -- and
- * a second memcpy: 1.1 GB/s, as slow as the whole GPU path is fast.) */
+ * (PyUnicode_AsUTF8AndSize would mean CPython's one-thread encoder plus a cached copy per string and a second memcpy.) */
 #include <pthread.h>
 
 typedef struct { const void *data; Py_ssize_t len; int kind; int ascii; } StrView;
@@ -134,7 +133,7 @@ fail:
 
 /* unpack(tokens_addr: int, offsets_addr: int, n_docs: int[, int_cache: list]) -> list[list[int]]
  * The reference converts Vec<Vec<Rank>> into Python lists of freshly made int objects (PyO3); making ~230 M ints per GiB
- * of text is what bounds the list-returning batch API on both sides (0.2 GB/s).  Token ids come from a vocabulary of
+ * of text is what bounds the list-returning batch API on both sides.  Token ids come from a vocabulary of
  * 50-200 k entries, so the int OBJECTS can be shared: `int_cache[i] is i` for every id, built once per encoding -- a token
  * then costs one table load and one reference count instead of an allocation. */
 static PyObject *unpack(PyObject *self, PyObject *args) {

@@ -61,12 +61,12 @@ B2_HD uint32_t b2_mad1(uint32_t v, uint32_t one, uint32_t c) {   // v * one + c 
     return v * one + c;
 #endif
 }
-// The byte tests of one (transposed) word.  Pipe balance matters more than the instruction count here: ncu shows the
-// kernel bound by the ALU pipe (LOP3 / SHF / IADD3: one warp instruction per two cycles and scheduler; 94 % busy in round 1)
-// while the FMA pipe, which executes IMAD, idles.  So the 15 per-byte comparisons of a word are written as multiply-adds
+// The byte tests of one (transposed) word.  Pipe balance matters more than the instruction count here: the kernel is
+// bound by the ALU pipe (LOP3 / SHF / IADD3: one warp instruction per two cycles and scheduler) while the FMA pipe,
+// which executes IMAD, idles.  So the 15 per-byte comparisons of a word are written as multiply-adds
 // (v * one + c with `one` == 1 at run time, opaque to the compiler -> IMAD); the combining logic and the accumulation
-// (one LEA.HI / SHF+LOP3 per class) stay on the ALU pipe.  A multiply-high accumulate (IMAD.HI) was measured too: it
-// moves more work off the ALU pipe but IMAD.HI issues at a quarter of the IMAD rate (profiles/r02_f_pretok_pipes.txt).
+// (one LEA.HI / SHF+LOP3 per class) stay on the ALU pipe.  A multiply-high accumulate (IMAD.HI) would
+// move more work off the ALU pipe, but IMAD.HI issues at a quarter of the IMAD rate.
 template <int K>
 B2_HD void classify_word(uint32_t x, ClassAcc &a, uint32_t one) {
     const uint32_t y = x & 0x7F7F7F7Fu, yl = y | 0x20202020u;

@@ -152,8 +152,8 @@ def gpu_numa_cpus(device_index: int) -> list[int] | None:
 
 def bind_to_gpu_numa(device_index: int) -> dict:
     """Pin this process to the CPUs next to its GPU BEFORE it allocates pinned host buffers: first touch then puts
-    them on that node, and H2D / D2H do not cross the inter-socket link (4 ranks sharing one node's memory halved the
-    PCIe rate in round 1).  Returns what was done, for the bench line."""
+    them on that node, and H2D / D2H do not cross the inter-socket link (ranks whose buffers sit on one node share that
+    node's memory and link bandwidth).  Returns what was done, for the bench line."""
     import os
     cpus = gpu_numa_cpus(device_index)
     if not cpus:
