@@ -147,7 +147,7 @@ int b200bpe_decode_batch(b200bpe_t *h, const uint32_t *tokens, const uint64_t *t
  * [7] count scan + gather, [8] probe kernel alone.  Also the kernel launch count. */
 int b200bpe_last_timings(b200bpe_t *h, float *ms9, uint32_t *n_launches);
 
-/* Sizes of the device tables (bytes) for reporting: [0] piece table, [1] pair table,
+/* Sizes of the device tables (bytes) for reporting: [0] piece tables (narrow + wide), [1] pair table,
  * [2] long-token table + blob, [3] Unicode class tables. */
 int b200bpe_table_bytes(b200bpe_t *h, uint64_t *bytes4);
 

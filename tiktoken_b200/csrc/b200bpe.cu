@@ -362,13 +362,15 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
     for (int i = 0; i < 128; i++) ascii[i] = UC_STAGE2[(uint32_t)UC_STAGE1[0] * 256 + i];
     // one arena, hottest tables first: the L2 persistence window covers a prefix of it
     struct Part { const void *src; size_t bytes; size_t off; };
-    Part parts[9] = {{H.piece_tab.data(), H.piece_tab.size() * sizeof(U4), 0}, {H.pair2.data(), 65536 * 4, 0},
-                     {H.byte_id.data(), 256 * 4, 0}, {H.pair_tab.data(), H.pair_tab.size() * sizeof(U4), 0},
-                     {ascii, 128, 0}, {UC_STAGE1, sizeof(UC_STAGE1), 0}, {UC_STAGE2, sizeof(UC_STAGE2), 0},
-                     {H.long_tab.data(), H.long_tab.size() * sizeof(U4), 0}, {H.long_blob.data(), H.long_blob.size(), 0}};
+    enum { P_NARROW, P_WIDE, P_PAIR2, P_BYTE_ID, P_PAIR, P_ASCII, P_UC1, P_UC2, P_LONG, P_BLOB, N_PARTS };
+    Part parts[N_PARTS] = {{H.narrow_tab.data(), H.narrow_tab.size() * sizeof(U4), 0},
+                           {H.wide_tab.data(), H.wide_tab.size() * sizeof(U4), 0}, {H.pair2.data(), 65536 * 4, 0},
+                           {H.byte_id.data(), 256 * 4, 0}, {H.pair_tab.data(), H.pair_tab.size() * sizeof(U4), 0},
+                           {ascii, 128, 0}, {UC_STAGE1, sizeof(UC_STAGE1), 0}, {UC_STAGE2, sizeof(UC_STAGE2), 0},
+                           {H.long_tab.data(), H.long_tab.size() * sizeof(U4), 0}, {H.long_blob.data(), H.long_blob.size(), 0}};
     size_t total = 0;
     for (auto &p : parts) { p.off = total; total += (p.bytes + 255) & ~(size_t)255; }
-    D->arena_bytes = total; D->hot_bytes = parts[4].off;
+    D->arena_bytes = total; D->hot_bytes = parts[P_ASCII].off;
     if (e == cudaSuccess) e = cudaMalloc((void **)&D->arena, total);
     for (auto &p : parts) if (e == cudaSuccess && p.bytes) e = cudaMemcpy(D->arena + p.off, p.src, p.bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMalloc((void **)&D->d_tok_boff, boff.size() * 4);
@@ -386,16 +388,17 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
         D->probe_blocks_per_sm = (int)env_long("B200BPE_PROBE_BLOCKS", 10, 1, 16);
     }
     if (e != cudaSuccess) { std::string m = cudaGetErrorString(e); devctx_destroy(D); return fail(B200BPE_ECUDA, "device " + std::to_string(device) + " setup: " + m); }
-    D->T.piece_tab = (const U4 *)(D->arena + parts[0].off); D->T.piece_mask = H.piece_mask;
-    D->T.pair2 = (const uint32_t *)(D->arena + parts[1].off);
-    D->T.byte_id = (const uint32_t *)(D->arena + parts[2].off);
-    D->T.pair_tab = (const U4 *)(D->arena + parts[3].off); D->T.pair_mask = H.pair_mask;
-    D->uc.ascii = D->arena + parts[4].off;
-    D->uc.stage1 = (const uint16_t *)(D->arena + parts[5].off);
-    D->uc.stage2 = D->arena + parts[6].off;
+    D->T.narrow_tab = (const U4 *)(D->arena + parts[P_NARROW].off); D->T.narrow_mask = H.narrow_mask;
+    D->T.wide_tab = (const U4 *)(D->arena + parts[P_WIDE].off); D->T.wide_mask = H.wide_mask;
+    D->T.pair2 = (const uint32_t *)(D->arena + parts[P_PAIR2].off);
+    D->T.byte_id = (const uint32_t *)(D->arena + parts[P_BYTE_ID].off);
+    D->T.pair_tab = (const U4 *)(D->arena + parts[P_PAIR].off); D->T.pair_mask = H.pair_mask;
+    D->uc.ascii = D->arena + parts[P_ASCII].off;
+    D->uc.stage1 = (const uint16_t *)(D->arena + parts[P_UC1].off);
+    D->uc.stage2 = D->arena + parts[P_UC2].off;
     D->uc.one = 1u;
-    D->T.long_tab = (const U4 *)(D->arena + parts[7].off); D->T.long_mask = H.long_mask;
-    D->T.long_blob = D->arena + parts[8].off;
+    D->T.long_tab = (const U4 *)(D->arena + parts[P_LONG].off); D->T.long_mask = H.long_mask;
+    D->T.long_blob = D->arena + parts[P_BLOB].off;
     D->T.max_token_len = H.max_token_len; D->T.n_long_tokens = H.n_long_tokens;
     // L2 persistence (off by default): a persisting access-policy window over the rank tables was measured on an H100
     // 80GB HBM3 (SXM, 700 W power limit) at 1 GiB per step -- cl100k English 120.8 GB/s without the window vs 64.6 with
@@ -490,7 +493,7 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
         bits = std::max(bits, 8);
         h->pack_bits = (bits <= 24 && env_long("B200BPE_PACK", 0, 0, 1)) ? bits : 0;   // opt-in: see DESIGN 4
     }
-    h->table_bytes[0] = H.piece_tab.size() * sizeof(U4);
+    h->table_bytes[0] = (H.narrow_tab.size() + H.wide_tab.size()) * sizeof(U4);
     h->table_bytes[1] = H.pair_tab.size() * sizeof(U4) + 65536 * 4 + 1024;
     h->table_bytes[2] = H.long_tab.size() * sizeof(U4) + H.long_blob.size();
     h->table_bytes[3] = sizeof(UC_STAGE1) + sizeof(UC_STAGE2) + 128;

@@ -8,14 +8,15 @@
 // Design (see DESIGN.md):
 //  * token id == rank.  A single byte the vocabulary lacks gets a pseudo id PSEUDO_BASE+byte so
 //    that merges through it still work; emitting one is the reference's panic (lib.rs:202,207).
-//  * PIECE table: open-addressed, 32-byte slots keyed by the piece bytes themselves
-//    (<= 16 bytes, two little-endian u64 + length) -> exact compare, one 32 B sector per probe.
+//  * PIECE tables: open-addressed, keyed by the piece bytes themselves -> exact compare.  Tokens of
+//    1..11 bytes go to the NARROW table, one 16-byte slot per probe step (key words + length + rank);
+//    tokens of 12..16 bytes to the WIDE table, 32-byte slots (key words, then length + rank).
 //  * LONG-token table: tokens > 16 bytes, keyed by a 64-bit hash, verified against a byte blob.
 //  * PAIR table: (id(A), id(B)) -> rank(A||B) for every split of every token into two parts that
 //    are themselves tokens (or single bytes).  Because every part produced by the merge loop is
 //    a token, probing bytes(A)||bytes(B) in the reference's map is the same as probing
 //    (id(A), id(B)) here -- fixed 8-byte keys, no variable-length hashing inside the loop
-//    (the reference's own remark, lib.rs:145-147 and :259-260).  16-byte slots.
+//    (the reference's own remark, lib.rs:145-147 and :259-260).  16-byte slots, probed one at a time.
 //  * PAIR2: direct 64 Ki-entry table for the initial byte pairs (lib.rs:149-155).
 #pragma once
 #include <stdint.h>
@@ -26,16 +27,21 @@ namespace b2bpe {
 static const uint32_t RANK_MAX = 0xFFFFFFFFu;
 static const uint32_t PSEUDO_BASE = 0xFFFFFE00u;   // ids >= this are "byte missing from vocabulary"
 static const int SHORT_MAX = 16;                   // pieces up to this length take the per-thread path
+static const uint32_t NARROW_MAX = 11;             // tokens up to this length live in the narrow piece table
+static const uint32_t PAIR_EMPTY = 0xFFFFFFFFu;    // `a` of an empty pair-table slot (no token id is this large)
+static const uint32_t PIECE_THROUGH = 0x80000000u; // pass-through mark in the rank word of a narrow piece slot
 
 struct U4 { uint32_t x, y, z, w; };                // host mirror of uint4
 
 struct DevTables {
     const uint32_t *byte_id;      // [256]
     const uint32_t *pair2;        // [65536] rank of the 2-byte token b0,b1 (index b0*256+b1) or RANK_MAX
-    const U4 *pair_tab;           // buckets of two slots {a, b, rank, 0}; empty slot: a == 0xFFFFFFFF
-    uint32_t pair_mask;           // number of buckets - 1
-    const U4 *piece_tab;          // 2 x U4 per slot: {k0lo,k0hi,k1lo,k1hi} {len, rank, 0, 0}; empty: len == 0
-    uint32_t piece_mask;
+    const U4 *pair_tab;           // one slot {a, b, rank, through} per probe step; empty slot: a == PAIR_EMPTY, through == 0
+    uint32_t pair_mask;           // number of slots - 1
+    const U4 *narrow_tab;         // tokens of 1..11 bytes, one U4 per slot: {w0, w1, w2 | len << 24, rank | through << 31}; empty: 0
+    uint32_t narrow_mask;
+    const U4 *wide_tab;           // tokens of 12..16 bytes, 2 x U4 per slot: {w0, w1, w2, w3} {len, rank, through, 0}; empty: 0
+    uint32_t wide_mask;
     const U4 *long_tab;           // 2 x U4 per slot: {hlo, hhi, blob_off, len} {rank,0,0,0}; empty: len == 0
     uint32_t long_mask;
     const uint8_t *long_blob;
@@ -50,18 +56,9 @@ __device__ __forceinline__ U4 ldg_u4(const U4 *p) {
     uint4 v = __ldg(reinterpret_cast<const uint4 *>(p));
     U4 r; r.x = v.x; r.y = v.y; r.z = v.z; r.w = v.w; return r;
 }
-// both 16-byte halves of a 32-byte table slot / bucket (one 32-byte sector).  sm_90 has no 256-bit load, so these are
-// two 128-bit loads issued back to back, both in flight before either result is used.
-__device__ __forceinline__ void ldg_u4x2(const U4 *p, U4 &a, U4 &b) {
-    asm("ld.global.nc.v4.u32 {%0,%1,%2,%3}, [%8];\n\t"
-        "ld.global.nc.v4.u32 {%4,%5,%6,%7}, [%8+16];"
-        : "=r"(a.x), "=r"(a.y), "=r"(a.z), "=r"(a.w), "=r"(b.x), "=r"(b.y), "=r"(b.z), "=r"(b.w) : "l"(p));
-}
-#define B2_LDG_U4X2(p, a, b) b2bpe::ldg_u4x2(p, a, b)
 #else
 #define B2_LDG_U4(p) (*(p))
 #define B2_LDG_U32(p) (*(p))
-#define B2_LDG_U4X2(p, a, b) do { (a) = (p)[0]; (b) = (p)[1]; } while (0)
 #endif
 
 B2_HD uint32_t pair_hash(uint32_t a, uint32_t b) {
@@ -100,52 +97,77 @@ B2_HD uint64_t long_hash_word(uint64_t w, uint32_t i) {
 B2_HD uint64_t long_hash_step(uint64_t h, uint64_t w, uint32_t i) { return h ^ long_hash_word(w, i); }
 B2_HD uint64_t long_hash_init(uint64_t len) { return len * 0xC2B2AE3D27D4EB4Full + 0x165667B19E3779F9ull; }
 
-// The pair table is probed in BUCKETS of two 16-byte slots (one 32-byte sector): both slots of a
-// bucket are loaded together, a bucket with a free slot ends the chain.  pair_mask = n_buckets - 1.
+// ---- pair table: linear probing over 16-byte slots {a, b, rank, through} ----------------------------------------
+// `through` is 1 when the probe path of some key passes the slot (bpe_tables.h): a slot that does not hold the key and is
+// not passed through -- an empty slot included -- ends the chain.
+// A probe is its start position, then steps: load the slot at s (pair_slot), look at it (pair_step).  Callers with
+// several probes load all their slots before they look at any, so the loads are in flight together.
+B2_HD uint32_t pair_start(const DevTables &T, uint32_t a, uint32_t b) { return pair_hash(a, b) & T.pair_mask; }
+B2_HD U4 pair_slot(const DevTables &T, uint32_t s) { return B2_LDG_U4(T.pair_tab + s); }
+// one probe step on the slot e loaded from position s: true when the chain ends (r = the rank, or RANK_MAX for an
+// absent pair), otherwise s moves to the next slot
+B2_HD bool pair_step(const DevTables &T, const U4 &e, uint32_t a, uint32_t b, uint32_t &s, uint32_t &r) {
+    if (e.x == a && e.y == b) { r = e.z; return true; }
+    if (e.w == 0) { r = RANK_MAX; return true; }
+    s = (s + 1) & T.pair_mask;
+    return false;
+}
+
 B2_HD uint32_t pair_lookup(const DevTables &T, uint32_t a, uint32_t b) {
-    uint32_t s = pair_hash(a, b) & T.pair_mask;
-    for (;;) {
-        U4 e0, e1; B2_LDG_U4X2(T.pair_tab + 2 * s, e0, e1);
-        if (e0.x == a && e0.y == b) return e0.z;
-        if (e1.x == a && e1.y == b) return e1.z;
-        if (e1.x == 0xFFFFFFFFu) return RANK_MAX;          // slots fill in order: a free second slot ends the chain
-        s = (s + 1) & T.pair_mask;
-    }
+    uint32_t s = pair_start(T, a, b), r = RANK_MAX;
+    while (!pair_step(T, pair_slot(T, s), a, b, s, r)) {}
+    return r;
 }
 
 // two independent pair probes with both first loads in flight together (the two neighbours of a
 // merge, src/lib.rs:182-185)
 B2_HD void pair_lookup2(const DevTables &T, uint32_t a1, uint32_t b1, uint32_t a2, uint32_t b2, uint32_t &r1,
                         uint32_t &r2) {
-    uint32_t s1 = pair_hash(a1, b1) & T.pair_mask, s2 = pair_hash(a2, b2) & T.pair_mask;
-    U4 e10, e11, e20, e21;
-    B2_LDG_U4X2(T.pair_tab + 2 * s1, e10, e11);
-    B2_LDG_U4X2(T.pair_tab + 2 * s2, e20, e21);
-    for (;;) {
-        if (e10.x == a1 && e10.y == b1) { r1 = e10.z; break; }
-        if (e11.x == a1 && e11.y == b1) { r1 = e11.z; break; }
-        if (e11.x == 0xFFFFFFFFu) { r1 = RANK_MAX; break; }
-        s1 = (s1 + 1) & T.pair_mask; B2_LDG_U4X2(T.pair_tab + 2 * s1, e10, e11);
-    }
-    for (;;) {
-        if (e20.x == a2 && e20.y == b2) { r2 = e20.z; break; }
-        if (e21.x == a2 && e21.y == b2) { r2 = e21.z; break; }
-        if (e21.x == 0xFFFFFFFFu) { r2 = RANK_MAX; break; }
-        s2 = (s2 + 1) & T.pair_mask; B2_LDG_U4X2(T.pair_tab + 2 * s2, e20, e21);
-    }
+    uint32_t s1 = pair_start(T, a1, b1), s2 = pair_start(T, a2, b2);
+    const U4 e1 = pair_slot(T, s1), e2 = pair_slot(T, s2);
+    if (!pair_step(T, e1, a1, b1, s1, r1)) while (!pair_step(T, pair_slot(T, s1), a1, b1, s1, r1)) {}
+    if (!pair_step(T, e2, a2, b2, s2, r2)) while (!pair_step(T, pair_slot(T, s2), a2, b2, s2, r2)) {}
 }
 
-// whole-piece probe for len <= 16 (src/lib.rs:367-368)
-B2_HD uint32_t piece_lookup16(const DevTables &T, uint64_t k0, uint64_t k1, uint32_t len) {
-    uint32_t s = (uint32_t)piece_hash(k0, k1, len) & T.piece_mask;
+// ---- piece tables: whole-piece probe for len <= 16 (src/lib.rs:367-368) ---------------------------------------
+// The key is the piece as four little-endian words a0..a3, zero padded beyond len.  The table depends on len only: a
+// narrow piece (len <= 11: byte 11 of its key is padding and carries len in the slot) loads one 16-byte slot per step, a
+// wide one both halves of a 32-byte slot.  As in the pair table, a slot carries a pass-through mark (bit 31 of a narrow
+// slot's rank word -- ranks are < 2^30 --, word z of a wide slot's second half): a slot that does not hold the key and is
+// not passed through ends the chain.  A probe is issued (first slot loaded) and finished (compare, continue the chain)
+// separately, so that a caller can keep several probes in flight.
+B2_HD void piece_load(const DevTables &T, uint32_t len, uint32_t s, U4 &e0, U4 &e1) {
+    const bool narrow = len <= NARROW_MAX;
+    const U4 *p = narrow ? T.narrow_tab + s : T.wide_tab + 2 * s;
+    e0 = B2_LDG_U4(p);
+    if (!narrow) e1 = B2_LDG_U4(p + 1);                      // e1 is not looked at for a narrow piece
+}
+// returns the probe position; e0 / e1 receive the slot there
+B2_HD uint32_t piece_issue(const DevTables &T, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t len,
+                           U4 &e0, U4 &e1) {
+    const uint32_t s = piece_hash4(a0, a1, a2, a3, len) & (len <= NARROW_MAX ? T.narrow_mask : T.wide_mask);
+    piece_load(T, len, s, e0, e1);
+    return s;
+}
+// the rank of the piece, or RANK_MAX; e0 / e1 is the slot at s that piece_issue loaded
+B2_HD uint32_t piece_finish(const DevTables &T, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t len,
+                            uint32_t s, U4 e0, U4 e1) {
+    const bool narrow = len <= NARROW_MAX;
+    const uint32_t mask = narrow ? T.narrow_mask : T.wide_mask;
+    const uint32_t z = narrow ? (a2 | len << 24) : a2;
     for (;;) {
-        U4 k, m; B2_LDG_U4X2(T.piece_tab + 2 * s, k, m);          // both halves of the 32-byte slot: one sector
-        if (m.x == 0) return RANK_MAX;
-        if (m.x == len && k.x == (uint32_t)k0 && k.y == (uint32_t)(k0 >> 32) && k.z == (uint32_t)k1 &&
-            k.w == (uint32_t)(k1 >> 32))
-            return m.y;
-        s = (s + 1) & T.piece_mask;
+        if (e0.x == a0 && e0.y == a1 && e0.z == z && (narrow || (e0.w == a3 && e1.x == len)))
+            return narrow ? e0.w & ~PIECE_THROUGH : e1.y;
+        if ((narrow ? e0.w & PIECE_THROUGH : e1.z) == 0) return RANK_MAX;   // no chain passes here (empty slots included)
+        s = (s + 1) & mask;
+        piece_load(T, len, s, e0, e1);
     }
+}
+B2_HD uint32_t piece_lookup16(const DevTables &T, uint64_t k0, uint64_t k1, uint32_t len) {
+    const uint32_t a0 = (uint32_t)k0, a1 = (uint32_t)(k0 >> 32), a2 = (uint32_t)k1, a3 = (uint32_t)(k1 >> 32);
+    U4 e0 = {0, 0, 0, 0}, e1 = {0, 0, 0, 0};
+    const uint32_t s = piece_issue(T, a0, a1, a2, a3, len, e0, e1);
+    return piece_finish(T, a0, a1, a2, a3, len, s, e0, e1);
 }
 
 // whole-piece probe for len > 16: hash already computed; bytes compared against the blob
@@ -300,25 +322,15 @@ B2_HD uint32_t merge_short_conv(const DevTables &T, ByteFn byte_at, int n, int n
             if (below) { need_l = true; jp = 31 - b2_clz(below); a2 = id[jp]; b2 = best; }
         }
         // the two neighbour probes of every active lane, issued together
-        uint32_t s1 = pair_hash(a1, b1) & T.pair_mask, s2 = pair_hash(a2, b2) & T.pair_mask;
+        uint32_t s1 = pair_start(T, a1, b1), s2 = pair_start(T, a2, b2);
         uint32_t r1 = RANK_MAX, r2 = RANK_MAX;
         bool p1 = need_r, p2 = need_l;
         while (B2_ANY(group, p1 || p2)) {
-            U4 e0 = {0, 0, 0, 0}, e1 = {0, 0, 0, 0}, f0 = {0, 0, 0, 0}, f1 = {0, 0, 0, 0};
-            if (p1) B2_LDG_U4X2(T.pair_tab + 2 * s1, e0, e1);
-            if (p2) B2_LDG_U4X2(T.pair_tab + 2 * s2, f0, f1);
-            if (p1) {
-                if (e0.x == a1 && e0.y == b1) { r1 = e0.z; p1 = false; }
-                else if (e1.x == a1 && e1.y == b1) { r1 = e1.z; p1 = false; }
-                else if (e1.x == 0xFFFFFFFFu) p1 = false;
-                else s1 = (s1 + 1) & T.pair_mask;
-            }
-            if (p2) {
-                if (f0.x == a2 && f0.y == b2) { r2 = f0.z; p2 = false; }
-                else if (f1.x == a2 && f1.y == b2) { r2 = f1.z; p2 = false; }
-                else if (f1.x == 0xFFFFFFFFu) p2 = false;
-                else s2 = (s2 + 1) & T.pair_mask;
-            }
+            U4 e = {0, 0, 0, 0}, f = {0, 0, 0, 0};
+            if (p1) e = pair_slot(T, s1);
+            if (p2) f = pair_slot(T, s2);
+            if (p1) p1 = !pair_step(T, e, a1, b1, s1, r1);
+            if (p2) p2 = !pair_step(T, f, a2, b2, s2, r2);
         }
         if (act) {
             rk[bj] = need_r ? r1 : RANK_MAX;
@@ -417,25 +429,15 @@ B2_HD void merge_mid_conv(const DevTables &T, int n, int n_max, unsigned group, 
             rk[j2] = link; rk[bj + 1] = link; rk[j3 - 1] = link;
         }
         // the two neighbour probes of every active lane, issued together
-        uint32_t s1 = pair_hash(a1, b1) & T.pair_mask, s2 = pair_hash(a2, b2) & T.pair_mask;
+        uint32_t s1 = pair_start(T, a1, b1), s2 = pair_start(T, a2, b2);
         uint32_t r1 = RANK_MAX, r2 = RANK_MAX;
         bool p1 = need_r, p2 = need_l;
         while (B2_ANY(group, p1 || p2)) {
-            U4 e0 = {0, 0, 0, 0}, e1 = {0, 0, 0, 0}, f0 = {0, 0, 0, 0}, f1 = {0, 0, 0, 0};
-            if (p1) B2_LDG_U4X2(T.pair_tab + 2 * s1, e0, e1);
-            if (p2) B2_LDG_U4X2(T.pair_tab + 2 * s2, f0, f1);
-            if (p1) {
-                if (e0.x == a1 && e0.y == b1) { r1 = e0.z; p1 = false; }
-                else if (e1.x == a1 && e1.y == b1) { r1 = e1.z; p1 = false; }
-                else if (e1.x == 0xFFFFFFFFu) p1 = false;
-                else s1 = (s1 + 1) & T.pair_mask;
-            }
-            if (p2) {
-                if (f0.x == a2 && f0.y == b2) { r2 = f0.z; p2 = false; }
-                else if (f1.x == a2 && f1.y == b2) { r2 = f1.z; p2 = false; }
-                else if (f1.x == 0xFFFFFFFFu) p2 = false;
-                else s2 = (s2 + 1) & T.pair_mask;
-            }
+            U4 e = {0, 0, 0, 0}, f = {0, 0, 0, 0};
+            if (p1) e = pair_slot(T, s1);
+            if (p2) f = pair_slot(T, s2);
+            if (p1) p1 = !pair_step(T, e, a1, b1, s1, r1);
+            if (p2) p2 = !pair_step(T, f, a2, b2, s2, r2);
         }
         if (act) {
             rk[bj] = need_r ? r1 : RANK_MAX;

@@ -60,7 +60,19 @@ extern "C" uint32_t hc_pair_lookup(void *p, uint32_t a, uint32_t b) {
     if (r != x || y != pair_lookup(T, b, a)) return 0xDEADBEEFu;
     return r;
 }
+// number of pair-table slots (one slot per probe step)
 extern "C" uint64_t hc_pair_buckets(void *p) { return (uint64_t)((HcTables *)p)->H.pair_mask + 1; }
+// whole-piece probe of 1..16 bytes (the probe kernel's issue / finish pair): rank or RANK_MAX
+extern "C" uint32_t hc_piece_lookup(void *p, const uint8_t *piece, uint32_t len) {
+    if (len == 0 || len > (uint32_t)SHORT_MAX) return 0xDEADBEEFu;
+    uint64_t k0, k1; pack16(piece, len, k0, k1);
+    return piece_lookup16(((HcTables *)p)->H.view(), k0, k1, len);
+}
+// slots of the narrow and the wide piece table
+extern "C" void hc_piece_slots(void *p, uint64_t *narrow, uint64_t *wide) {
+    const HostTables &H = ((HcTables *)p)->H;
+    *narrow = H.narrow_tab.size(); *wide = H.wide_tab.size() / 2;
+}
 
 // the short path of the encode kernel for one piece of 1..16 bytes: whole-piece probe
 // (lib.rs:367-368) then merge_short; ids >= PSEUDO_BASE are reported as RANK_MAX.

@@ -3,8 +3,8 @@
 // probe_kernel   persistent warps, one 1 KiB sub-tile at a time: the TMA unit stages the next sub-tile's text and
 //                piece-start words into shared memory (cp.async.bulk + mbarrier, double buffered) while the warp works
 //                on the current one; the piece starts are compacted into a list (all 32 lanes busy whatever the
-//                distribution) and every piece of <= 16 bytes is probed in the piece table (src/lib.rs:367-368), two
-//                probes in flight per lane.  One 32-bit slot per PIECE goes to `ptok` (token id, or a tagged reference
+//                distribution) and every piece of <= 16 bytes is probed in the piece tables (src/lib.rs:367-368), two
+//                probes in flight per lane: one 16-byte load per step for a piece of <= 11 bytes, two above.  One 32-bit slot per PIECE goes to `ptok` (token id, or a tagged reference
 //                to the miss queue / the long-piece queue); a miss is appended to a global queue TOGETHER WITH ITS 16
 //                KEY BYTES, so that nothing downstream goes back to the text.
 // miss_*         counting sort of the misses by piece length, carrying the records; miss_kernel: one piece per lane,
@@ -82,25 +82,26 @@ __global__ void __launch_bounds__(ENC_WARPS * 32) probe_kernel(TileParams p, Dev
     const long long stride = (long long)gridDim.x * ENC_WARPS;
     long long sub = (long long)blockIdx.x * ENC_WARPS + (threadIdx.x >> 5);
     if (sub >= p.n_sub) return;                          // warps are independent: no block barrier below
-    const uint32_t mb[2] = {smem_u32(&S.mbar[0]), smem_u32(&S.mbar[1])};
-    const uint32_t s_text[2] = {smem_u32(S.text[0]), smem_u32(S.text[1])};
-    const uint32_t s_pw[2] = {smem_u32(S.p[0]), smem_u32(S.p[1])};
+    // shared-memory addresses of buffer b are base + b * size: computed, not taken from an array indexed by the run-time
+    // buffer number (such an array lives in local memory)
+    const uint32_t mb0 = smem_u32(&S.mbar[0]), s_text0 = smem_u32(S.text[0]), s_pw0 = smem_u32(S.p[0]);
+    auto mb = [&](int b) -> uint32_t { return mb0 + (uint32_t)b * (uint32_t)sizeof(S.mbar[0]); };
     const uint64_t pol = l2_policy_evict_first();        // the text is streamed once: do not let it displace the tables in L2
-    if (lane == 0) { mbar_init(mb[0], 1); mbar_init(mb[1], 1); mbar_fence_init(); }
+    if (lane == 0) { mbar_init(mb(0), 1); mbar_init(mb(1), 1); mbar_fence_init(); }
     __syncwarp();
     // TMA staging of sub-tile t into buffer b (lane 0): text (readable up to n_bytes + 16) and piece-start words
     auto stage = [&](long long t, int b) {
         const long long left = p.n_bytes - t * SUB_BYTES;
         const uint32_t tbytes = left >= STAGE_TEXT ? (uint32_t)STAGE_TEXT : (uint32_t)((left + 15) & ~15ll);
-        mbar_arrive_expect_tx(mb[b], tbytes + STAGE_PW * 4);
-        if (tbytes) tma_load_1d(s_text[b], p.text + t * SUB_BYTES, tbytes, mb[b], pol);
-        tma_load_1d(s_pw[b], p.pbits + t * 32, STAGE_PW * 4, mb[b], pol);
+        mbar_arrive_expect_tx(mb(b), tbytes + STAGE_PW * 4);
+        if (tbytes) tma_load_1d(s_text0 + (uint32_t)b * (uint32_t)sizeof(S.text[0]), p.text + t * SUB_BYTES, tbytes, mb(b), pol);
+        tma_load_1d(s_pw0 + (uint32_t)b * (uint32_t)sizeof(S.p[0]), p.pbits + t * 32, STAGE_PW * 4, mb(b), pol);
     };
     if (lane == 0) stage(sub, 0);
     int cur = 0; uint32_t phase = 0;                      // bit b of `phase` = parity to wait for on buffer b
     for (; sub < p.n_sub; sub += stride, cur ^= 1) {
         if (lane == 0 && sub + stride < p.n_sub) stage(sub + stride, cur ^ 1);   // overlaps with this sub-tile's probes
-        mbar_wait(mb[cur], (phase >> cur) & 1u);
+        mbar_wait(mb(cur), (phase >> cur) & 1u);
         phase ^= 1u << cur;
         const uint8_t *txt = S.text[cur];
         const uint32_t *pw = S.p[cur];
@@ -153,14 +154,8 @@ __global__ void __launch_bounds__(ENC_WARPS * 32) probe_kernel(TileParams p, Dev
             load_key(txt, off, len, a0, a1, a2, a3);
             return 1;
         };
-        auto finish = [&](uint32_t i, int len, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t s, U4 m, U4 k) {
-            uint32_t r = RANK_MAX;
-            for (;;) {                                         // continue the linear probe from the prefetched slot
-                if (m.x == 0) break;
-                if (m.x == (uint32_t)len && k.x == a0 && k.y == a1 && k.z == a2 && k.w == a3) { r = m.y; break; }
-                s = (s + 1) & T.piece_mask;
-                B2_LDG_U4X2(T.piece_tab + 2 * s, k, m);
-            }
+        auto finish = [&](uint32_t i, int len, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t s, U4 e0, U4 e1) {
+            const uint32_t r = piece_finish(T, a0, a1, a2, a3, (uint32_t)len, s, e0, e1);   // continues from the prefetched slot
             if (r != RANK_MAX) { st_stream_u32(slot + i, r); cnt++; }
             else S.miss[atomicAdd(&S.nmiss, 1u)] = (uint16_t)i;
         };
@@ -170,11 +165,11 @@ __global__ void __launch_bounds__(ENC_WARPS * 32) probe_kernel(TileParams p, Dev
             const int needA = prep(i, lenA, a0, a1, a2, a3);
             const int needB = prep(i + 32, lenB, b0, b1, b2, b3);
             uint32_t sA = 0, sB = 0;
-            U4 mA = {0, 0, 0, 0}, kA = {0, 0, 0, 0}, mB = {0, 0, 0, 0}, kB = {0, 0, 0, 0};
-            if (needA) { sA = piece_hash4(a0, a1, a2, a3, (uint32_t)lenA) & T.piece_mask; B2_LDG_U4X2(T.piece_tab + 2 * sA, kA, mA); }
-            if (needB) { sB = piece_hash4(b0, b1, b2, b3, (uint32_t)lenB) & T.piece_mask; B2_LDG_U4X2(T.piece_tab + 2 * sB, kB, mB); }
-            if (needA) finish(i, lenA, a0, a1, a2, a3, sA, mA, kA);
-            if (needB) finish(i + 32, lenB, b0, b1, b2, b3, sB, mB, kB);
+            U4 eA0 = {0, 0, 0, 0}, eA1 = {0, 0, 0, 0}, eB0 = {0, 0, 0, 0}, eB1 = {0, 0, 0, 0};
+            if (needA) sA = piece_issue(T, a0, a1, a2, a3, (uint32_t)lenA, eA0, eA1);
+            if (needB) sB = piece_issue(T, b0, b1, b2, b3, (uint32_t)lenB, eB0, eB1);
+            if (needA) finish(i, lenA, a0, a1, a2, a3, sA, eA0, eA1);
+            if (needB) finish(i + 32, lenB, b0, b1, b2, b3, sB, eB0, eB1);
         }
         __syncwarp();
 

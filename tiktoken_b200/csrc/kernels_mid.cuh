@@ -174,16 +174,9 @@ __device__ void midg_class(const uint8_t *__restrict__ text, const DevTables &T,
             if (DUAL && gl == 3 && need_l2) { a = S.id[at(jpb)]; b = best2; pr = true; }
             uint32_t r = RANK_MAX;
             {
-                uint32_t sidx = pair_hash(a, b) & T.pair_mask;
-                while (__any_sync(0xFFFFFFFFu, pr)) {
-                    if (pr) {
-                        U4 e0, e1; B2_LDG_U4X2(T.pair_tab + 2 * sidx, e0, e1);
-                        if (e0.x == a && e0.y == b) { r = e0.z; pr = false; }
-                        else if (e1.x == a && e1.y == b) { r = e1.z; pr = false; }
-                        else if (e1.x == 0xFFFFFFFFu) pr = false;
-                        else sidx = (sidx + 1) & T.pair_mask;
-                    }
-                }
+                uint32_t sidx = pair_start(T, a, b);
+                while (__any_sync(0xFFFFFFFFu, pr))
+                    if (pr) pr = !pair_step(T, pair_slot(T, sidx), a, b, sidx, r);
             }
             const uint32_t r1r = __shfl_sync(0xFFFFFFFFu, r, gb), r1l = __shfl_sync(0xFFFFFFFFu, r, gb + 1);
             uint32_t r2r = RANK_MAX, r2l = RANK_MAX;
