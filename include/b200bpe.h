@@ -147,6 +147,17 @@ int b200bpe_decode_batch(b200bpe_t *h, const uint32_t *tokens, const uint64_t *t
  * [7] count scan + gather, [8] probe kernel alone.  Also the kernel launch count. */
 int b200bpe_last_timings(b200bpe_t *h, float *ms9, uint32_t *n_launches);
 
+/* What the most recent encode call on this handle had to redo: `grown` = OR of B200BPE_GREW_* for the work-spaces this
+ * call grew and re-ran, `reruns` = pipeline re-runs summed over chunks and devices, `token_passes` = 1, or 2 when the
+ * host token buffer had to be re-sized.  Every encode entry point, b200bpe_encode_device_async and b200bpe_device_wait
+ * included, resets all three to 0 first, so a call that fails early reports zeros.  A work-space that was too small for
+ * an EARLIER call of a queued device series is not grown (that series fails with B200BPE_ECAPACITY) and is not in
+ * `grown`. */
+#define B200BPE_GREW_MISS 1u   /* miss queue or miss result space */
+#define B200BPE_GREW_SLOW 2u   /* undecided pre-tokeniser positions */
+#define B200BPE_GREW_LONG 4u   /* long-piece merge scratch */
+int b200bpe_last_reruns(b200bpe_t *h, uint32_t *grown, uint32_t *reruns, uint32_t *token_passes);
+
 /* Sizes of the device tables (bytes) for reporting: [0] piece tables (narrow + wide), [1] pair table,
  * [2] long-token table + blob, [3] Unicode class tables. */
 int b200bpe_table_bytes(b200bpe_t *h, uint64_t *bytes4);

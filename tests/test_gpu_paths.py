@@ -28,15 +28,17 @@ def _oracle(ranks, special, pat):
     return Oracle(ranks, special, pat)
 
 
-def _chunked_encoding(enc_name, chunk_mb, **env):
-    """An Encoding whose host pipeline cuts batches into chunk_mb-MiB chunks (knobs are read at construction)."""
+def _chunked_encoding(enc_name, chunk_mb, vocab=None, devices=None, **env):
+    """An Encoding whose host pipeline cuts batches into chunk_mb-MiB chunks (knobs are read at construction).
+    vocab = (pat_str, mergeable_ranks, special_tokens) replaces the named synthetic encoding; devices as Encoding's."""
     import tiktoken_b200
-    pat, ranks, special, _ = vu.load_encoding(enc_name, allow_real=False)
+    pat, ranks, special = vocab or vu.load_encoding(enc_name, allow_real=False)[:3]
     env = dict(env, B200BPE_CHUNK_MB=chunk_mb)
     old = {k: os.environ.get(k) for k in env}
     os.environ.update({k: str(v) for k, v in env.items()})
     try:
-        e = tiktoken_b200.Encoding(enc_name + "_chunk", pat_str=pat, mergeable_ranks=ranks, special_tokens=special)
+        e = tiktoken_b200.Encoding(f"{enc_name}_chunk", pat_str=pat, mergeable_ranks=ranks, special_tokens=special,
+                                   devices=devices)
     finally:
         for k, v in old.items():
             if v is None:

@@ -350,6 +350,16 @@ class CoreBPE:
         d["launches"] = int(n.value)
         return d
 
+    def last_reruns(self) -> dict:
+        """What the most recent encode call had to redo: `grown` names the work-spaces it grew and re-ran ("miss",
+        "slow", "long"), `reruns` counts pipeline re-runs over all chunks and devices, `token_passes` is 2 when the
+        host token buffer had to be re-sized.  Every encode call, `encode_device_async` included, starts from zeros."""
+        grown, reruns, passes = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        _lib.check(self._L.b200bpe_last_reruns(self._h, C.byref(grown), C.byref(reruns), C.byref(passes)))
+        names = {_lib.GREW_MISS: "miss", _lib.GREW_SLOW: "slow", _lib.GREW_LONG: "long"}
+        return {"grown": {s for bit, s in names.items() if grown.value & bit}, "reruns": int(reruns.value),
+                "token_passes": int(passes.value)}
+
     def trim(self) -> None:
         """Give the engine's grow-only device work-spaces and pooled pinned blocks back (tables stay)."""
         _lib.check(self._L.b200bpe_trim(self._h))

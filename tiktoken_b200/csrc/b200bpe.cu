@@ -281,6 +281,10 @@ struct b200bpe {
     uint64_t table_bytes[4] = {0, 0, 0, 0};
     float last_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     uint32_t last_launches = 0;
+    // what the most recent encode call had to redo (b200bpe_last_reruns); reset by every encode entry point, before its
+    // argument checks and outside h->mu, hence atomic
+    std::atomic<uint32_t> last_grown{0}, last_reruns{0}, last_token_passes{0};
+    void reset_reruns() { last_grown = 0; last_reruns = 0; last_token_passes = 0; }
     size_t chunk_bytes = 64u << 20; bool chunk_forced = false;
     int copy_threads = 4;
     TaskPool *pool = nullptr;        // helper threads (created with the first host-path call)
@@ -762,8 +766,9 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
 static const int B200BPE_RETRY = 1;      // internal: capacities were grown, run the pipeline again
 
 // Wait for an enqueued pipeline, collect stage timings and device-side flags.  Returns B200BPE_RETRY when a
-// work-space that is sized from experience was too small for this batch (it has been grown to the exact need).
-static int collect_pipeline(b200bpe *h, Slot &S, int *special_idx, uint64_t *special_pos) {
+// work-space that is sized from experience was too small for this batch (it has been grown to the exact need);
+// the B200BPE_GREW_* bits of the work-spaces that grew are then ORed into *grown.
+static int collect_pipeline(b200bpe *h, Slot &S, int *special_idx, uint64_t *special_pos, uint32_t *grown) {
     (void)h;
     CUDA_TRY(cudaEventSynchronize(S.ev[9]));
     CUDA_TRY(cudaGetLastError());
@@ -790,6 +795,8 @@ static int collect_pipeline(b200bpe *h, Slot &S, int *special_idx, uint64_t *spe
             S.miss_cap = std::max(S.miss_cap, (size_t)c.n_miss + (size_t)(c.n_miss / 8) + 4096);
             S.mres_cap = std::max(S.mres_cap, (size_t)c.miss_bytes + (size_t)(c.miss_bytes / 8) + 4096);
         }
+        *grown |= ((c.err & ERR_MISSCAP) ? B200BPE_GREW_MISS : 0u) | ((c.err & ERR_SLOWCAP) ? B200BPE_GREW_SLOW : 0u) |
+                  ((c.err & ERR_LONGCAP) ? B200BPE_GREW_LONG : 0u);
         return B200BPE_RETRY;
     }
     if (c.err & ERR_INTERNAL) return fail(B200BPE_ECUDA, "internal error: a merge kernel did not converge");
@@ -824,6 +831,7 @@ static int device_enqueue_locked(b200bpe *h, const PendingDeviceCall &c) {
 extern "C" int b200bpe_encode_device_async(b200bpe_t *h, const uint8_t *d_text, uint64_t n_bytes, const uint64_t *d_doc_off,
                                            uint64_t n_docs, uint32_t *d_tokens, uint64_t *d_tok_off, uint64_t *d_counts,
                                            void *stream) {
+    if (h) h->reset_reruns();
     int rc = device_args_check(h, d_text, n_bytes, d_doc_off, d_tokens, d_tok_off);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(h->mu);
@@ -842,6 +850,7 @@ extern "C" int b200bpe_encode_device_async(b200bpe_t *h, const uint8_t *d_text, 
 
 extern "C" int b200bpe_device_wait(b200bpe_t *h, uint64_t *n_tokens) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
+    h->reset_reruns();
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->pending.active) return fail(B200BPE_EINVAL, "no device call in flight");
     DeviceGuard guard;
@@ -850,8 +859,11 @@ extern "C" int b200bpe_device_wait(b200bpe_t *h, uint64_t *n_tokens) {
     Slot &S = D->slots[0];
     PendingDeviceCall c = h->pending;
     h->pending.active = false;
+    h->last_token_passes = 1;
     cudaStream_t st = c.st ? c.st : S.stream;
-    int rc = collect_pipeline(h, S, nullptr, nullptr);
+    uint32_t grown = 0;                   // only what this wait grows: an earlier call of a queued series leaves sticky bits
+    int rc = collect_pipeline(h, S, nullptr, nullptr, &grown);
+    h->last_grown = grown;
     const uint64_t total = S.h_ctr->total_tokens;
     // error bits of the earlier calls of a queued series (the counters only describe the last one)
     unsigned int sticky = 0;
@@ -863,7 +875,9 @@ extern "C" int b200bpe_device_wait(b200bpe_t *h, uint64_t *n_tokens) {
     for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {
         rc = device_enqueue_locked(h, c);
         if (rc) break;
-        rc = collect_pipeline(h, S, nullptr, nullptr);
+        h->last_reruns++;
+        rc = collect_pipeline(h, S, nullptr, nullptr, &grown);
+        h->last_grown = grown;
         total2 = S.h_ctr->total_tokens;
         CUDA_TRY(cudaMemsetAsync(S.d_sticky, 0, sizeof(unsigned int), st));
         reran = true;
@@ -907,6 +921,7 @@ struct HostJob {
     std::string error_msg; std::mutex err_mu;
     int special_idx = -1; uint64_t special_pos = 0;
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; std::mutex stat_mu;
+    uint32_t grown = 0, reruns = 0;               // B200BPE_GREW_* bits / pipeline re-runs of all workers (under stat_mu)
 
     void set_error(int rc) {
         std::lock_guard<std::mutex> lk(err_mu);
@@ -1012,16 +1027,17 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     };
     size_t known = 0; uint64_t known_sum = 0;                    // prefix of the per-chunk token counts seen so far
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; float last_d2h = 0;
+    uint32_t grown = 0, reruns = 0;
     // finalise chunk k: wait for its kernels, then send its offsets + tokens home (async) at their final place
     auto drain = [&](size_t k) -> int {
         Slot &S = slot_of(k);
         const size_t c = mine[k];
         const uint64_t lo = J->cut[c], hi = J->cut[c + 1], nd = hi - lo;
         int sidx = -1; uint64_t spos = 0;
-        int rc = collect_pipeline(h, S, &sidx, &spos);
+        int rc = collect_pipeline(h, S, &sidx, &spos, &grown);
         for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {   // a work-space grew: same chunk again
             rc = enqueue_pipeline(h, D, S, args_of(k));
-            if (!rc) rc = collect_pipeline(h, S, &sidx, &spos);
+            if (!rc) { reruns++; rc = collect_pipeline(h, S, &sidx, &spos, &grown); }
         }
         if (rc == B200BPE_RETRY) rc = fail(B200BPE_ECUDA, "work-space sizing did not converge");
         if (rc == B200BPE_ESPECIAL) {
@@ -1090,6 +1106,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     for (int i = 0; i < 9; i++) J->sum_ms[i] = std::max(J->sum_ms[i], sum_ms[i]);       // per device; report the slowest
     J->sum_ms[6] = std::max(J->sum_ms[6], last_d2h);
     J->launches += launches;
+    J->grown |= grown; J->reruns += reruns;
 }
 
 static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, bool single_piece,
@@ -1149,6 +1166,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
             for (int d = 0; d < workers; d++) th.emplace_back(host_worker, &J, d, (size_t)d, (size_t)workers);
             for (auto &t : th) t.join();
         }
+        h->last_grown |= J.grown; h->last_reruns += J.reruns; h->last_token_passes = (uint32_t)pass + 1;
         if (J.error.load()) {
             g_last_error = J.error_msg;
             if (J.error.load() == B200BPE_ESPECIAL && special_idx) *special_idx = J.special_idx;
@@ -1168,6 +1186,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
 
 extern "C" int b200bpe_encode_ordinary_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off,
                                              uint64_t n_docs, b200bpe_result_t **out) {
+    if (h) h->reset_reruns();
     if (!h || !doc_off || !out) return fail(B200BPE_EINVAL, "null argument");
     if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
     std::lock_guard<std::mutex> lk(h->mu);
@@ -1176,6 +1195,7 @@ extern "C" int b200bpe_encode_ordinary_batch(b200bpe_t *h, const uint8_t *text, 
 }
 
 extern "C" int b200bpe_encode_single_piece(b200bpe_t *h, const uint8_t *piece, uint64_t len, b200bpe_result_t **out) {
+    if (h) h->reset_reruns();
     if (!h || !out || (len && !piece)) return fail(B200BPE_EINVAL, "null argument");
     std::lock_guard<std::mutex> lk(h->mu);
     DeviceGuard guard;
@@ -1189,6 +1209,7 @@ extern "C" int b200bpe_encode_single_piece(b200bpe_t *h, const uint8_t *piece, u
 // emitted as their own ids.  flags[i]: 1 = allowed, 2 = disallowed, 0 = ordinary text.
 extern "C" int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                             const uint8_t *flags, b200bpe_result_t **out, int32_t *special_index) {
+    if (h) h->reset_reruns();
     if (!h || !doc_off || !out) return fail(B200BPE_EINVAL, "null argument");
     if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
     bool any = false;
@@ -1204,6 +1225,7 @@ extern "C" int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, c
 extern "C" int b200bpe_encode_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                     const uint8_t *allowed, b200bpe_result_t **out) {
     if (!h) return fail(B200BPE_EINVAL, "null argument");
+    h->reset_reruns();
     std::vector<uint8_t> flags(h->specials.size() + 1, 0);
     if (allowed) for (size_t i = 0; i < h->specials.size(); i++) flags[i] = allowed[i] ? 1 : 0;
     return b200bpe_encode_batch_special(h, text, doc_off, n_docs, allowed ? flags.data() : nullptr, out, nullptr);
@@ -1366,6 +1388,14 @@ extern "C" int b200bpe_last_timings(b200bpe_t *h, float *ms9, uint32_t *n_launch
     if (!h) return fail(B200BPE_EINVAL, "null handle");
     if (ms9) memcpy(ms9, h->last_ms, sizeof(h->last_ms));
     if (n_launches) *n_launches = h->last_launches;
+    return B200BPE_OK;
+}
+
+extern "C" int b200bpe_last_reruns(b200bpe_t *h, uint32_t *grown, uint32_t *reruns, uint32_t *token_passes) {
+    if (!h) return fail(B200BPE_EINVAL, "null handle");
+    if (grown) *grown = h->last_grown.load();
+    if (reruns) *reruns = h->last_reruns.load();
+    if (token_passes) *token_passes = h->last_token_passes.load();
     return B200BPE_OK;
 }
 
