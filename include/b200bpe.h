@@ -158,6 +158,14 @@ int b200bpe_last_timings(b200bpe_t *h, float *ms9, uint32_t *n_launches);
 #define B200BPE_GREW_LONG 4u   /* long-piece merge scratch */
 int b200bpe_last_reruns(b200bpe_t *h, uint32_t *grown, uint32_t *reruns, uint32_t *token_passes);
 
+/* Which long-piece merge kernels the most recent encode call on this handle ran: counts[c] = pieces of length class c
+ * (0: 17..32, 1: 33..64, 2: 65..128, 3: 129..256, 4: 257..1024, 5: 1025..4096, 6: 4097..32768, 7: longer bytes),
+ * summed over chunks and devices, from the runs whose output the call returned; *lane_per_piece = 1 when the
+ * lane-per-piece kernels merged them (largest rank 2^22 or above), 0 for the group and parallel-merge kernels.  After
+ * a queued device series the counts describe its last call.  Reset to zeros where b200bpe_last_reruns is, and left at
+ * zeros by a call that fails. */
+int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *lane_per_piece);
+
 /* Sizes of the device tables (bytes) for reporting: [0] piece tables (narrow + wide), [1] pair table,
  * [2] long-token table + blob, [3] Unicode class tables. */
 int b200bpe_table_bytes(b200bpe_t *h, uint64_t *bytes4);

@@ -34,6 +34,15 @@ def test_unsupported_pattern_is_value_error():
         _tiktoken.CoreBPE({bytes([i]): i for i in range(256)}, {}, r"\w+|\s+")   # no CPU regex fallback
 
 
+def test_special_token_id_of_2_pow_30_is_value_error():
+    """Token ids must be below 2^30, special ones included (the probe kernel tags token slots with the top two bits);
+    checked before the device is touched."""
+    from tiktoken_b200 import _tiktoken
+    ranks = {bytes([i]): i for i in range(256)}
+    with pytest.raises(ValueError, match="special token id too large"):
+        _tiktoken.CoreBPE(ranks, {"<|endoftext|>": 1 << 30}, vu.CL100K_PAT)
+
+
 @pytest.mark.skipif(have_gpu(), reason="checks the no-GPU failure mode")
 def test_no_gpu_fails_loudly_not_silently():
     from tiktoken_b200 import _tiktoken

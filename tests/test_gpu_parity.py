@@ -215,44 +215,3 @@ def test_device_decode_batch_roundtrip_and_errors():
     assert e.decode_bytes_batch([]) == [] and e.decode_bytes_batch([[], []]) == [b"", b""]
     with pytest.raises(KeyError):
         e.decode_bytes_batch([[1, 2, 10 ** 7]])
-
-
-def test_mid_piece_length_classes_with_adversarial_vocabulary():
-    """Pieces of 17..1100 bytes that are NOT tokens, on a tiny-alphabet vocabulary full of rank ties and
-    cascades (random, periodic and long-run shapes), batched so that every length class -- group of lanes 17-32 / 33-64 /
-    65-128, segmented parallel merge 129-256 (two pieces per batch) and 257-1024 (one), warp per piece beyond -- sees
-    full, ragged and single-piece batches, including the class boundaries."""
-    import random
-    import tiktoken_b200
-    from oracle import Oracle
-    rnd = random.Random(77)
-    for trial in range(3):
-        alpha = "abc"[: 2 + trial % 2] + "de"
-        ranks = {bytes([i]): i for i in range(256)}
-        toks = set()
-        for _ in range(60):
-            toks.add("".join(rnd.choice(alpha) for _ in range(rnd.choice([2, 2, 2, 3, 3, 4, 5, 7, 12, 20, 40]))).encode())
-        for t, r in zip(sorted(toks), rnd.sample(range(256, 1000), len(toks))):
-            ranks[t] = r
-        e = tiktoken_b200.Encoding("adv_mid", pat_str=vu.CL100K_PAT, mergeable_ranks=ranks, special_tokens={})
-        o = Oracle(ranks, {}, vu.CL100K_PAT)
-        lens = [16, 17, 18, 31, 32, 33, 34, 63, 64, 65, 66, 127, 128, 129, 130, 200, 255, 256, 257, 258, 300,
-                400, 511, 512, 513, 700, 1023, 1024, 1025, 1100]
-        words = []
-        for n in lens:
-            for _ in range(rnd.choice([1, 5, 33, 70]) if n <= 300 else rnd.choice([1, 2, 7])):
-                style = rnd.choice(["random", "random", "periodic", "runs"])      # equal-rank chains and cascades too
-                if style == "random":
-                    w = "".join(rnd.choice(alpha) for _ in range(n))
-                elif style == "periodic":
-                    unit = "".join(rnd.choice(alpha) for _ in range(rnd.choice([1, 2, 3, 5])))
-                    w = (unit * (n // len(unit) + 1))[:n]
-                else:
-                    w = ""
-                    while len(w) < n:
-                        w += rnd.choice(alpha) * rnd.choice([1, 2, 3, 9, 40])
-                    w = w[:n]
-                words.append(w)
-        rnd.shuffle(words)
-        docs = [" ".join(words), " ".join(words[::3]), words[0], ""]      # letters+ pieces split at the spaces
-        assert e.encode_ordinary_batch(docs) == [o.encode_ordinary(d) for d in docs]

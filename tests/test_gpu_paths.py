@@ -284,26 +284,6 @@ def test_device_special_scan_edge_cases():
         assert buf.tokens().tolist() == flat
 
 
-def test_ranks_of_2_pow_24_and_above_take_the_lane_per_piece_kernel():
-    """Token ids beyond 24 bits cannot be packed into the group kernel's keys: those vocabularies run the
-    one-piece-per-lane kernel (and decode through the host maps)."""
-    import tiktoken_b200
-    rnd = random.Random(3)
-    ranks = {bytes([i]): i for i in range(256)}
-    toks = set()
-    while len(toks) < 50:
-        toks.add("".join(rnd.choice("abcd") for _ in range(rnd.choice([2, 2, 3, 4, 6, 9, 20]))).encode())
-    for t, r in zip(sorted(toks), rnd.sample(range(1 << 24, (1 << 24) + 5000), len(toks))):
-        ranks[t] = r
-    e = tiktoken_b200.Encoding("big_ranks", pat_str=vu.CL100K_PAT, mergeable_ranks=ranks, special_tokens={"<|x|>": (1 << 25)})
-    o = _oracle(ranks, {"<|x|>": 1 << 25}, vu.CL100K_PAT)
-    words = ["".join(rnd.choice("abcd") for _ in range(n)) for n in (5, 17, 31, 33, 64, 65, 128, 200, 256, 257, 300) for _ in range(9)]
-    docs = [" ".join(words), words[20], "<|x|>".join(words[:5])]
-    got = e.encode_batch(docs, allowed_special="all")
-    assert got == [o.encode(d, {"<|x|>"}) for d in docs]
-    assert e.decode_batch(got) == docs
-
-
 def test_queued_device_calls_and_count_buffer():
     import torch
     import tiktoken_b200

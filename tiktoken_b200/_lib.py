@@ -96,6 +96,8 @@ def lib() -> C.CDLL:
     L.b200bpe_last_timings.argtypes = [vp, vp, C.POINTER(u32)]
     L.b200bpe_last_reruns.restype = i32
     L.b200bpe_last_reruns.argtypes = [vp, C.POINTER(u32), C.POINTER(u32), C.POINTER(u32)]
+    L.b200bpe_last_piece_classes.restype = i32
+    L.b200bpe_last_piece_classes.argtypes = [vp, vp, C.POINTER(i32)]
     L.b200bpe_table_bytes.restype = i32
     L.b200bpe_table_bytes.argtypes = [vp, vp]
     L.b200bpe_device_count.restype = i32
@@ -113,6 +115,7 @@ EXPORTS = [
     "b200bpe_decode_bytes", "b200bpe_decode_batch", "b200bpe_last_timings", "b200bpe_table_bytes", "b200bpe_last_error",
     "b200bpe_version", "b200bpe_device_count", "b200bpe_create_multi", "b200bpe_n_devices", "b200bpe_encode_batch_special",
     "b200bpe_special_name", "b200bpe_encode_device_async", "b200bpe_device_wait", "b200bpe_trim", "b200bpe_last_reruns",
+    "b200bpe_last_piece_classes",
 ]
 
 GREW_MISS, GREW_SLOW, GREW_LONG = 1, 2, 4       # B200BPE_GREW_* (b200bpe_last_reruns)

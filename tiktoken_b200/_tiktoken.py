@@ -360,6 +360,15 @@ class CoreBPE:
         return {"grown": {s for bit, s in names.items() if grown.value & bit}, "reruns": int(reruns.value),
                 "token_passes": int(passes.value)}
 
+    def last_piece_classes(self) -> dict:
+        """Which long-piece merge kernels the most recent encode call ran: `counts[c]` = pieces of length class c
+        (17..32, 33..64, 65..128, 129..256, 257..1024, 1025..4096, 4097..32768 and more bytes) of the runs whose output
+        it returned, `lane_per_piece` = the lane-per-piece kernels of vocabularies with ranks of 2^22 and above merged
+        them.  Zeros after a call that failed."""
+        counts, lane = (C.c_uint64 * 8)(), C.c_int32(0)
+        _lib.check(self._L.b200bpe_last_piece_classes(self._h, counts, C.byref(lane)))
+        return {"counts": [int(x) for x in counts], "lane_per_piece": bool(lane.value)}
+
     def trim(self) -> None:
         """Give the engine's grow-only device work-spaces and pooled pinned blocks back (tables stay)."""
         _lib.check(self._L.b200bpe_trim(self._h))

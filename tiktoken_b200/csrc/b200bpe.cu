@@ -284,7 +284,19 @@ struct b200bpe {
     // what the most recent encode call had to redo (b200bpe_last_reruns); reset by every encode entry point, before its
     // argument checks and outside h->mu, hence atomic
     std::atomic<uint32_t> last_grown{0}, last_reruns{0}, last_token_passes{0};
-    void reset_reruns() { last_grown = 0; last_reruns = 0; last_token_passes = 0; }
+    // long pieces per length class of the runs whose output the most recent encode call returned, and whether the
+    // lane-per-piece kernels merged them (b200bpe_last_piece_classes); reset with the re-run counters
+    std::atomic<uint64_t> last_cls[N_CLS] = {};
+    std::atomic<int> last_lane_per_piece{0};
+    void reset_reruns() {
+        last_grown = 0; last_reruns = 0; last_token_passes = 0;
+        for (auto &c : last_cls) c = 0;
+        last_lane_per_piece = 0;
+    }
+    void set_piece_classes(const uint64_t *cls) {
+        for (int c = 0; c < N_CLS; c++) last_cls[c] = cls[c];
+        last_lane_per_piece = mid_group ? 0 : 1;
+    }
     size_t chunk_bytes = 64u << 20; bool chunk_forced = false;
     int copy_threads = 4;
     TaskPool *pool = nullptr;        // helper threads (created with the first host-path call)
@@ -438,6 +450,10 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
     else return fail(B200BPE_EPATTERN,
                      "unsupported pat_str: the GPU pre-tokeniser implements exactly the r50k/p50k, cl100k and "
                      "o200k patterns of tiktoken_ext/openai_public.py (there is no CPU regex fallback)");
+    // the probe kernel tags a piece's token slot with the top two bits (kernels_encode.cuh PT_KIND), special ids included:
+    // like the mergeable ranks (build_tables), every special id must stay below them
+    for (uint32_t i = 0; i < n_sp; i++)
+        if (sp_rank[i] >= (1u << 30)) return fail(B200BPE_EINVAL, "special token id too large (token ids must be < 2^30)");
     int ndev = 0;
     if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) {
         cudaGetLastError();
@@ -895,6 +911,9 @@ extern "C" int b200bpe_device_wait(b200bpe_t *h, uint64_t *n_tokens) {
         if (sticky & ERR_DOCOFF) return fail(B200BPE_EINVAL, "malformed document offsets in a queued device call");
     }
     if (n_tokens) *n_tokens = total2;
+    uint64_t cls[N_CLS];                  // the last call of a queued series: the counters describe that one
+    for (int k = 0; k < N_CLS; k++) cls[k] = S.h_ctr->n_cls[k];
+    h->set_piece_classes(cls);
     return B200BPE_OK;
 }
 
@@ -922,6 +941,7 @@ struct HostJob {
     int special_idx = -1; uint64_t special_pos = 0;
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; std::mutex stat_mu;
     uint32_t grown = 0, reruns = 0;               // B200BPE_GREW_* bits / pipeline re-runs of all workers (under stat_mu)
+    uint64_t cls[N_CLS] = {};                     // long pieces per length class of the chunks' final runs (under stat_mu)
 
     void set_error(int rc) {
         std::lock_guard<std::mutex> lk(err_mu);
@@ -1028,6 +1048,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     size_t known = 0; uint64_t known_sum = 0;                    // prefix of the per-chunk token counts seen so far
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; float last_d2h = 0;
     uint32_t grown = 0, reruns = 0;
+    uint64_t cls[N_CLS] = {};
     // finalise chunk k: wait for its kernels, then send its offsets + tokens home (async) at their final place
     auto drain = [&](size_t k) -> int {
         Slot &S = slot_of(k);
@@ -1048,6 +1069,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         if (rc) return rc;
         float h2d = 0; cudaEventElapsedTime(&h2d, S.ev[5], S.ev[6]);
         const uint64_t nt = S.h_ctr->total_tokens;
+        for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
         J->count[c].store((long long)nt);
         while (known < c) {                                      // token base = counts of all earlier chunks (other devices)
             long long v = J->count[known].load();
@@ -1107,6 +1129,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     J->sum_ms[6] = std::max(J->sum_ms[6], last_d2h);
     J->launches += launches;
     J->grown |= grown; J->reruns += reruns;
+    for (int i = 0; i < N_CLS; i++) J->cls[i] += cls[i];
 }
 
 static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, bool single_piece,
@@ -1177,6 +1200,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
         for (auto &c : J.count) total += (uint64_t)std::max<long long>(0, c.load());
         memcpy(h->last_ms, J.sum_ms, sizeof(J.sum_ms)); h->last_launches = J.launches;
         r->n_tokens = total;
+        h->set_piece_classes(J.cls);
         h->live_results++;                                        // caller holds h->mu
         *out = r;
         return B200BPE_OK;
@@ -1396,6 +1420,13 @@ extern "C" int b200bpe_last_reruns(b200bpe_t *h, uint32_t *grown, uint32_t *reru
     if (grown) *grown = h->last_grown.load();
     if (reruns) *reruns = h->last_reruns.load();
     if (token_passes) *token_passes = h->last_token_passes.load();
+    return B200BPE_OK;
+}
+
+extern "C" int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *lane_per_piece) {
+    if (!h) return fail(B200BPE_EINVAL, "null handle");
+    if (counts8) for (int c = 0; c < N_CLS; c++) counts8[c] = h->last_cls[c].load();
+    if (lane_per_piece) *lane_per_piece = h->last_lane_per_piece.load();
     return B200BPE_OK;
 }
 
