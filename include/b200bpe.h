@@ -93,6 +93,17 @@ int b200bpe_encode_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_
 int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                  const uint8_t *flags, b200bpe_result_t **out, int32_t *special_index);
 
+/* CoreBPE::_encode_bytes (src/py.rs:72-115, Encoding._encode_bytes in tiktoken/core.py) for every document of a batch:
+ * the documents need not be UTF-8.  A document that is well-formed UTF-8 gets exactly the tokens of
+ * b200bpe_encode_ordinary_batch.  For any other, with v = its std::str::from_utf8 valid_up_to: its first v bytes are
+ * encoded as their own haystack (special-token text is ordinary text), the tokens of their last regex piece are dropped
+ * (together with the all-space tokens before them when the first of them is all-space, lib.rs:444-481) and the dropped
+ * bytes plus everything from v on are encoded as ONE piece (whole-piece probe, then byte_pair_encode).  A missing
+ * single-byte token fails with B200BPE_ENOBYTE.  Same buffers and result as b200bpe_encode_ordinary_batch.  Needs every
+ * token id below 2^24 (the device decode tables give the token lengths), else B200BPE_EINVAL. */
+int b200bpe_encode_bytes_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
+                               b200bpe_result_t **out);
+
 /* Name of special token `index` (as given to b200bpe_create), or NULL. */
 const char *b200bpe_special_name(b200bpe_t *h, int32_t index);
 
@@ -165,6 +176,10 @@ int b200bpe_last_reruns(b200bpe_t *h, uint32_t *grown, uint32_t *reruns, uint32_
  * a queued device series the counts describe its last call.  Reset to zeros where b200bpe_last_reruns is, and left at
  * zeros by a call that fails. */
 int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *lane_per_piece);
+
+/* Documents the most recent b200bpe_encode_bytes_batch call on this handle found not to be well-formed UTF-8 and
+ * repaired, summed over chunks and devices.  0 after any other encode call and after a call that failed. */
+int b200bpe_last_bytes_repairs(b200bpe_t *h, uint64_t *n_docs_repaired);
 
 /* Sizes of the device tables (bytes) for reporting: [0] piece tables (narrow + wide), [1] pair table,
  * [2] long-token table + blob, [3] Unicode class tables. */

@@ -195,6 +195,20 @@ class CoreBPE:
         _lib.check(rc)
         return TokenBuffer(self._L, res, self)
 
+    def encode_bytes_batch_buffer(self, text: np.ndarray, doc_off: np.ndarray) -> TokenBuffer:
+        """CoreBPE::_encode_bytes (src/py.rs:72-115) for every document: text uint8[N] need not be UTF-8, doc_off
+        uint64[n_docs+1] -> TokenBuffer.  Well-formed documents get exactly the tokens of encode_ordinary_batch_buffer;
+        KeyError when an unstable piece needs a single byte the vocabulary lacks."""
+        res = C.c_void_p()
+        rc = self._L.b200bpe_encode_bytes_batch(self._h, _ptr(text if len(text) else np.zeros(1, np.uint8)), _ptr(doc_off),
+                                                len(doc_off) - 1, C.byref(res))
+        _lib.check(rc)
+        return TokenBuffer(self._L, res, self)
+
+    def encode_bytes_batch(self, docs: list[bytes]) -> list[list[int]]:
+        text, off = _flatten_bytes([bytes(d) for d in docs])
+        return self._unpack(self.encode_bytes_batch_buffer(text, off))
+
     @staticmethod
     def _pack(texts: list[str]):
         """list[str] -> (uint8 blob, uint64 offsets); UnicodeEncodeError on lone surrogates, like the
@@ -368,6 +382,13 @@ class CoreBPE:
         counts, lane = (C.c_uint64 * 8)(), C.c_int32(0)
         _lib.check(self._L.b200bpe_last_piece_classes(self._h, counts, C.byref(lane)))
         return {"counts": [int(x) for x in counts], "lane_per_piece": bool(lane.value)}
+
+    def last_bytes_repairs(self) -> int:
+        """Documents the most recent encode_bytes_batch* call found not to be well-formed UTF-8 and repaired (0 after any
+        other call)."""
+        n = C.c_uint64(0)
+        _lib.check(self._L.b200bpe_last_bytes_repairs(self._h, C.byref(n)))
+        return int(n.value)
 
     def trim(self) -> None:
         """Give the engine's grow-only device work-spaces and pooled pinned blocks back (tables stay)."""

@@ -9,7 +9,9 @@ What this file adds to the inherited class, and nothing else:
     whole batch instead of a ThreadPoolExecutor over per-document calls (core.py:161-203, :334-350); `num_threads`
     is accepted and ignored (the GPU is the pool); the disallowed-special check of `encode_batch` runs inside the same
     device scan that cuts the documents at allowed specials, instead of a Python regex search per document;
-  * array-returning variants (`*_to_numpy`, `*_packed`) that never build Python lists.
+  * array-returning variants (`*_to_numpy`, `*_packed`) that never build Python lists;
+  * `encode_bytes_batch` / `encode_bytes_packed`: the reference's `_encode_bytes` (src/py.rs:72-115) for a batch of
+    documents that need not be UTF-8, on the device.
 For a process that should run the UNMODIFIED reference package on the GPU engine, see `tiktoken_b200.install()`.
 """
 from __future__ import annotations
@@ -172,6 +174,17 @@ class Encoding(_ref_core.Encoding):
                                                       disallowed_special or ())
         except _tiktoken.DisallowedSpecial as e:
             _ref_core.raise_disallowed_special_token(e.token)
+
+    def encode_bytes_batch(self, data: Sequence[bytes], *, num_threads: int = 8) -> list[list[int]]:
+        """`_encode_bytes` (core.py:406-407, src/py.rs:72-115) of every document, in one native call: a document that is
+        not UTF-8 is encoded up to its first ill-formed byte, and the tokens of that prefix's last piece are re-encoded
+        together with the rest of the document as one piece."""
+        return self._core_bpe.encode_bytes_batch(list(data))
+
+    def encode_bytes_packed(self, data: np.ndarray, doc_off: np.ndarray):
+        """`encode_bytes_batch` on packed input: uint8[N] (any bytes) + uint64[n_docs+1] -> zero-copy TokenBuffer."""
+        return self._core_bpe.encode_bytes_batch_buffer(np.ascontiguousarray(data, np.uint8),
+                                                        np.ascontiguousarray(doc_off, np.uint64))
 
     # ---------------------------------------------------------------- batch decode: one native call
     def decode_batch(self, batch: Sequence[Sequence[int]], *, errors: str = "replace", num_threads: int = 8) -> list[str]:

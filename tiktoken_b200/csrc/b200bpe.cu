@@ -20,6 +20,8 @@
 //                         warp-convergent exact min-rank merge on dense records
 //   scan_{partial,top,final}, gather_kernel, big_copy_kernel   token counts -> offsets -> tokens and
 //                         per-document offsets at their final place
+//   utf8_check, bytes_*   (bytes mode only, kernels_bytes.cuh) documents that are not well-formed UTF-8: cut at the
+//                         first ill-formed byte, repair of the last piece, a second run over the unstable pieces, splice
 //
 // No tensor cores: nothing here is a contraction.  The work is byte/integer, bound by HBM reads
 // of the text, L2 probes of the rank tables and instruction issue.
@@ -53,6 +55,7 @@
 #include "kernels_encode.cuh"
 #include "kernels_special.cuh"
 #include "kernels_decode.cuh"
+#include "kernels_bytes.cuh"
 #include "unicode_classes.inc"
 
 using namespace b2bpe;
@@ -175,6 +178,12 @@ struct Slot {
     DevBuf<unsigned long long> w_lq_start, w_lq_off; DevBuf<unsigned int> w_lq_len, w_lq_ntok, w_lq_cls, w_big_n, w_sort_hist;
     DevBuf<unsigned long long> w_big_dst, w_big_src, w_scan_part;
     DevBuf<uint32_t> w_idA, w_rkA, w_idB, w_rkB, w_aux1, w_aux2; DevBuf<uint8_t> w_flag, w_spflags;
+    // bytes mode: first ill-formed byte (then unstable-piece start), tokens to drop and tail bytes per document; run 2's
+    // text, document offsets and output; the spliced result (swapped with w_out / w_tokoff)
+    DevBuf<uint32_t> w_vup, w_kdrop, w_btail, w_b2out, w_bout; DevBuf<uint8_t> w_btext;
+    DevBuf<unsigned long long> w_b2doc, w_b2off, w_bbase, w_bpart;
+    // allocated by the first bytes-mode call: the splice's scan (run 2 reuses d_ctr), the repair's counters (h_bytes pinned)
+    Counters *d_bctr = nullptr; BytesCounters *d_bytes = nullptr, *h_bytes = nullptr;
     size_t long_cap = 0;            // entries of the global merge scratch (pieces > 256 bytes), grown on ERR_LONGCAP
     size_t miss_cap = 0, mres_cap = 0;   // miss queue entries / miss result tokens, grown on ERR_MISSCAP
     size_t slow_cap = 0;            // positions left to the general pre-tokeniser rule function, grown on ERR_SLOWCAP
@@ -184,7 +193,8 @@ struct Slot {
     cudaStream_t side = nullptr;     // the group kernels (17..1024 bytes) run here, next to probe + miss on the main stream,
     cudaStream_t side2 = nullptr;    // and the scratch kernels (warp / block / cluster per piece: a few SMs each) here
     cudaStream_t up = nullptr;       // host path: uploads of the slot's NEXT chunk (ordered behind the kernels, not the download, of its last one)
-    static const int N_EV = 15;       // [10] fork, [11] side start, [12] side end (join), [13] side2 end (join), [14] packed tokens on the host
+    static const int N_EV = 16;       // [10] fork, [11] side start, [12] side end (join), [13] side2 end (join), [14] packed tokens on the host,
+                                      // [15] bytes mode: start of the tail runs
     cudaEvent_t ev[N_EV];
     PinnedBuf stage;                // pinned staging for callers whose text is pageable memory
     DevBuf<uint32_t> w_pack;        // bit-packed tokens of the chunk (host path)
@@ -217,6 +227,8 @@ struct Slot {
         w_sort_hist.release(); w_big_dst.release(); w_big_src.release(); w_scan_part.release();
         w_idA.release(); w_rkA.release(); w_idB.release(); w_rkB.release(); w_aux1.release(); w_aux2.release();
         w_flag.release(); w_pack.release();
+        w_vup.release(); w_kdrop.release(); w_btail.release(); w_b2out.release(); w_bout.release(); w_btext.release();
+        w_b2doc.release(); w_b2off.release(); w_bbase.release(); w_bpart.release();
         if (stage.p) cudaFreeHost(stage.p);
         stage.p = nullptr; stage.cap = 0;
         if (stage_out.p) cudaFreeHost(stage_out.p);
@@ -226,6 +238,9 @@ struct Slot {
     void destroy() {
         release_workspace();
         if (d_ctr) cudaFree(d_ctr);
+        if (d_bctr) cudaFree(d_bctr);
+        if (d_bytes) cudaFree(d_bytes);
+        if (h_bytes) cudaFreeHost(h_bytes);
         if (d_sticky) cudaFree(d_sticky);
         if (h_ctr) cudaFreeHost(h_ctr);
         if (ok) { for (int i = 0; i < N_EV; i++) cudaEventDestroy(ev[i]); }
@@ -245,6 +260,8 @@ struct DevCtx {
     uint8_t *arena = nullptr; size_t arena_bytes = 0, hot_bytes = 0;   // all tables in one allocation (one L2 window)
     DevTables T; UcTables uc;
     uint32_t *d_tok_boff = nullptr; uint8_t *d_tok_blob = nullptr;     // decode: id -> bytes
+    uint32_t *d_tok_space = nullptr;                                   // bit per id: every byte is ' ', '\n' or '\t' (uploaded by
+                                                                       // the first bytes-mode call)
     SpecialTables sp;                                                  // device copy of the special-token patterns
     uint8_t *d_sp_arena = nullptr;
     static const int N_SLOTS = B2_N_SLOTS;
@@ -277,6 +294,7 @@ struct b200bpe {
     std::unordered_map<uint32_t, std::string> special_decoder;
     SpecialHost sp_host;                // hash table of the specials (built once), uploaded to every device
     uint32_t n_ids = 0; bool decode_on_device = true;
+    std::vector<uint32_t> tok_space;    // bit per id: all-space token (bytes mode; each device gets a copy on first use)
     std::vector<DevCtx *> devs;
     uint64_t table_bytes[4] = {0, 0, 0, 0};
     float last_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -288,8 +306,9 @@ struct b200bpe {
     // lane-per-piece kernels merged them (b200bpe_last_piece_classes); reset with the re-run counters
     std::atomic<uint64_t> last_cls[N_CLS] = {};
     std::atomic<int> last_lane_per_piece{0};
+    std::atomic<uint64_t> last_bytes_repairs{0};   // documents the most recent bytes-mode call repaired (b200bpe_last_bytes_repairs)
     void reset_reruns() {
-        last_grown = 0; last_reruns = 0; last_token_passes = 0;
+        last_grown = 0; last_reruns = 0; last_token_passes = 0; last_bytes_repairs = 0;
         for (auto &c : last_cls) c = 0;
         last_lane_per_piece = 0;
     }
@@ -351,6 +370,7 @@ static void devctx_destroy(DevCtx *D) {
     if (D->arena) cudaFree(D->arena);
     if (D->d_tok_boff) cudaFree(D->d_tok_boff);
     if (D->d_tok_blob) cudaFree(D->d_tok_blob);
+    if (D->d_tok_space) cudaFree(D->d_tok_space);
     if (D->d_sp_arena) cudaFree(D->d_sp_arena);
     delete D;
 }
@@ -483,13 +503,20 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
     h->n_ids = any ? max_id + 1 : 0;
     std::vector<uint32_t> boff((size_t)h->n_ids + 2, 0);
     std::vector<uint8_t> blob;
+    std::vector<uint32_t> &space = h->tok_space;
+    space.assign((size_t)h->n_ids / 32 + 2, 0);                  // token_is_all_space of lib.rs:455-465, per id
     for (uint32_t id = 0; id < h->n_ids; id++) {
         boff[id] = (uint32_t)blob.size();
         const std::string *sp = nullptr;
         auto it = H.decoder.find(id);
         if (it != H.decoder.end()) sp = &it->second;
         else { auto it2 = h->special_decoder.find(id); if (it2 != h->special_decoder.end()) sp = &it2->second; }
-        if (sp) blob.insert(blob.end(), sp->begin(), sp->end());
+        if (sp) {
+            blob.insert(blob.end(), sp->begin(), sp->end());
+            bool all = !sp->empty();
+            for (char c : *sp) all &= c == ' ' || c == '\n' || c == '\t';
+            if (all) space[id >> 5] |= 1u << (id & 31);
+        }
     }
     boff[h->n_ids] = (uint32_t)blob.size(); boff[h->n_ids + 1] = (uint32_t)blob.size();
     if (blob.empty()) blob.push_back(0);
@@ -577,7 +604,8 @@ struct PipeArgs {
     uint32_t *d_out = nullptr; unsigned long long *d_tok_off = nullptr;
     unsigned long long *d_counts = nullptr;      // optional device u64[2]: {n_tokens, n_docs} (for a count exchange)
     cudaStream_t st = nullptr;
-    bool single_piece = false;
+    bool single_piece = false;                   // every document is one piece (P = D)
+    bool bytes = false;                          // bytes mode: documents need not be UTF-8 (kernels_bytes.cuh)
     const uint8_t *sp_flags = nullptr;           // host: per special 1 = allowed, 2 = disallowed (NULL: no special handling)
 };
 
@@ -678,15 +706,39 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
                                                      S.w_hbits.p, S.w_ibits.p, S.w_sbits.p, S.w_ltok.p, n_words, S.d_ctr);
         launches += 2;
         hbits = S.w_hbits.p; ibits = S.w_ibits.p; sbits = S.w_sbits.p;
+    } else if (a.bytes) {
+        // ordinary semantics, so the special scan does not run and the cut owns its buffers: a document whose first
+        // ill-formed byte is v gets a haystack start at v and one placeholder slot for (v, end), like an accepted special
+        if (!D->d_tok_space) {
+            CUDA_TRY(cudaMalloc((void **)&D->d_tok_space, h->tok_space.size() * 4));
+            CUDA_TRY(cudaMemcpy(D->d_tok_space, h->tok_space.data(), h->tok_space.size() * 4, cudaMemcpyHostToDevice));
+        }
+        if (!S.d_bytes) CUDA_TRY(cudaMalloc((void **)&S.d_bytes, sizeof(BytesCounters)));
+        if (!S.h_bytes) CUDA_TRY(cudaHostAlloc((void **)&S.h_bytes, sizeof(BytesCounters), cudaHostAllocPortable));
+        CUDA_TRY(cudaMemsetAsync(S.d_bytes, 0, sizeof(BytesCounters), st));
+        CUDA_TRY(S.w_hbits.ensure((size_t)n_words + 8)); CUDA_TRY(S.w_ibits.ensure((size_t)n_words + 8));
+        CUDA_TRY(S.w_sbits.ensure((size_t)n_words + 8)); CUDA_TRY(S.w_vup.ensure((size_t)n_docs + 2));
+        CUDA_TRY(cudaMemsetAsync(S.w_ibits.p, 0, ((size_t)n_words + 8) * 4, st));
+        CUDA_TRY(cudaMemsetAsync(S.w_sbits.p, 0, ((size_t)n_words + 8) * 4, st));
+        CUDA_TRY(cudaMemsetAsync(S.w_vup.p, 0xFF, ((size_t)n_docs + 2) * 4, st));
+        utf8_check_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(a.d_text, (long long)n_bytes, S.w_dbits.p, S.w_sfd.p,
+                                                                            a.d_doc_off, n_docs, n_words, S.w_vup.p);
+        CUDA_TRY(cudaMemcpyAsync(S.w_hbits.p, S.w_dbits.p, ((size_t)n_words + 8) * 4, cudaMemcpyDeviceToDevice, st));
+        if (n_docs) bytes_cut_kernel<<<(unsigned)((n_docs * 32 + 255) / 256), 256, 0, st>>>(a.d_doc_off, n_docs, S.w_vup.p, S.w_hbits.p,
+                                                                                          S.w_ibits.p, S.w_sbits.p, S.w_ltok.p);
+        launches += 2;
+        hbits = S.w_hbits.p; ibits = S.w_ibits.p; sbits = S.w_sbits.p;
     }
     CUDA_TRY(cudaEventRecord(S.ev[1], st));
     {
         unsigned grid = (unsigned)((n_words + 255) / 256);
-        if (a.single_piece) single_piece_bits_kernel<<<grid, 256, 0, st>>>(S.w_pbits.p, S.w_psum.p, (long long)n_bytes, n_words);
+        if (a.single_piece) single_piece_bits_kernel<<<grid, 256, 0, st>>>(S.w_pbits.p, S.w_psum.p, S.w_dbits.p, n_words);
         else {
             const uint32_t scap = (uint32_t)std::min<size_t>(S.slow_cap, 0xFFFFFFF0u);
 #define B2_PRETOK(P)                                                                                                                   \
-    pretok_kernel<P><<<grid, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, n_words, ibits,          \
+    if (a.bytes) pretok_kernel<P, true><<<grid, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p,       \
+                                                             n_words, ibits, S.w_slow.p, scap, S.d_ctr);                              \
+    else pretok_kernel<P><<<grid, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, n_words, ibits,          \
                                           S.w_slow.p, scap, S.d_ctr);                                                                  \
     pretok_slow_kernel<P><<<D->n_sm * 8, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, S.w_slow.p, scap, S.d_ctr)
             if (h->pattern == PAT_R50K) { B2_PRETOK(PAT_R50K); }
@@ -769,10 +821,18 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
             gather_kernel<1><<<(unsigned)((n_docs + 1 + GATHER_WARPS - 1) / GATHER_WARPS), GATHER_WARPS * 32, 0, st>>>(p);
         } else gather_kernel<2><<<gather_grid, GATHER_WARPS * 32, 0, st>>>(p);
         big_copy_kernel<<<D->n_sm * 2, 256, 0, st>>>(p);
+        if (a.bytes && n_docs) {     // the tokens and offsets are final: where each damaged document's unstable piece starts
+            CUDA_TRY(S.w_kdrop.ensure((size_t)n_docs + 2)); CUDA_TRY(S.w_btail.ensure((size_t)n_docs + 2));
+            bytes_repair_kernel<<<(unsigned)((n_docs * 32 + 255) / 256), 256, 0, st>>>(a.d_doc_off, n_docs, S.w_vup.p, S.w_pbits.p, a.d_out,
+                                                                                      a.d_tok_off, D->d_tok_boff, D->d_tok_space, h->n_ids,
+                                                                                      S.w_kdrop.p, S.w_btail.p, S.d_bytes, S.d_ctr);
+            launches++;
+        }
         finalize_kernel<<<1, 32, 0, st>>>(S.d_ctr, S.d_sticky, a.d_counts, n_docs);
         launches += sparse_docs ? 12 : 11;
     }
     CUDA_TRY(cudaEventRecord(S.ev[4], st));
+    if (a.bytes) CUDA_TRY(cudaMemcpyAsync(S.h_bytes, S.d_bytes, sizeof(BytesCounters), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(S.h_ctr, S.d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaEventRecord(S.ev[9], st));
     S.last_launches = launches;
@@ -925,13 +985,71 @@ extern "C" int b200bpe_encode_device(b200bpe_t *h, const uint8_t *d_text, uint64
     return b200bpe_device_wait(h, n_tokens);
 }
 
+// exclusive scan of n u32 counts into base[0..n] (base[n] = the sum, also in ctr->total_tokens), on st
+static void enqueue_scan(const uint32_t *cnt, uint64_t n, unsigned long long *part, unsigned long long *base, Counters *ctr,
+                         cudaStream_t st) {
+    const long long nb = (long long)((n + SCAN_ITEMS - 1) / SCAN_ITEMS);
+    scan_partial_kernel<<<(unsigned)nb, 256, 0, st>>>(cnt, (long long)n, part);
+    scan_top_kernel<<<1, 1024, 0, st>>>(part, nb, ctr);
+    scan_final_kernel<<<(unsigned)nb, 256, 0, st>>>(cnt, (long long)n, part, base, ctr);
+}
+
+// Bytes mode, a chunk whose run 1 (a1, counters in S.h_ctr and S.h_bytes) found documents that are not well-formed UTF-8: run 2 encodes
+// the unstable piece [u_d, end_d) of every such document as one piece, then the splice puts each document's run-1 tokens
+// minus the last kdrop[d] in front of its run-2 tokens.  The final tokens and offsets end up in S.w_out / S.w_tokoff and
+// *nt is their count.  Run 2 is sized from run 1's counters, which the host already waited for: that is the one extra
+// round trip of a damaged chunk.
+static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, uint64_t *nt, uint64_t *cls, uint32_t *grown,
+                           uint32_t *reruns) {
+    const uint64_t n1 = S.h_ctr->total_tokens, drop = S.h_bytes->drop;
+    const float ms1[9] = {S.last_ms[0], S.last_ms[1], S.last_ms[2], S.last_ms[3], S.last_ms[4], S.last_ms[5], S.last_ms[6],
+                          S.last_ms[7], S.last_ms[8]};
+    const uint32_t launches1 = S.last_launches;
+    const uint64_t nd = a1.n_docs, tail = S.h_bytes->tail;
+    cudaStream_t st = a1.st;
+    CUDA_TRY(S.w_b2doc.ensure((size_t)nd + 2)); CUDA_TRY(S.w_b2off.ensure((size_t)nd + 2)); CUDA_TRY(S.w_bbase.ensure((size_t)nd + 2));
+    CUDA_TRY(S.w_bpart.ensure((size_t)(nd / SCAN_ITEMS) + 4));
+    CUDA_TRY(S.w_btext.ensure((size_t)tail + 64)); CUDA_TRY(S.w_b2out.ensure((size_t)tail + 64));
+    if (!S.d_bctr) CUDA_TRY(cudaMalloc((void **)&S.d_bctr, sizeof(Counters)));
+    CUDA_TRY(cudaEventRecord(S.ev[15], st));
+    enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_b2doc.p, S.d_bctr, st);
+    bytes_gather_kernel<<<(unsigned)((tail + 16 * 256 - 1) / (16 * 256)), 256, 0, st>>>(a1.d_text, nd, S.w_vup.p, S.w_b2doc.p, S.w_btext.p);
+    PipeArgs a2;
+    a2.d_text = S.w_btext.p; a2.n_bytes = tail; a2.d_doc_off = S.w_b2doc.p; a2.n_docs = nd;
+    a2.d_out = S.w_b2out.p; a2.d_tok_off = S.w_b2off.p; a2.st = st; a2.single_piece = true;
+    int rc = enqueue_pipeline(h, D, S, a2);
+    if (!rc) rc = collect_pipeline(h, S, nullptr, nullptr, grown);
+    for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {   // a work-space grew: run 2 again
+        rc = enqueue_pipeline(h, D, S, a2);
+        if (!rc) { (*reruns)++; rc = collect_pipeline(h, S, nullptr, nullptr, grown); }
+    }
+    if (rc == B200BPE_RETRY) rc = fail(B200BPE_ECUDA, "work-space sizing did not converge");
+    if (rc) return rc;
+    float ms2 = 0; cudaEventElapsedTime(&ms2, S.ev[15], S.ev[4]);
+    for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
+    const uint32_t launches2 = S.last_launches;
+    *nt = n1 - drop + S.h_ctr->total_tokens;
+    CUDA_TRY(S.w_bout.ensure((size_t)std::max<uint64_t>(*nt, a1.n_bytes) + 64));
+    bytes_count_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, st>>>(S.w_tokoff.p, S.w_b2off.p, S.w_kdrop.p, nd, S.w_btail.p);
+    enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_bbase.p, S.d_bctr, st);
+    bytes_splice_kernel<<<(unsigned)std::min<uint64_t>(nd, (uint64_t)D->n_sm * 16), 256, 0, st>>>(
+        S.w_out.p, S.w_tokoff.p, S.w_b2out.p, S.w_b2off.p, S.w_kdrop.p, S.w_bbase.p, nd, S.w_bout.p);
+    CUDA_TRY(cudaGetLastError());
+    std::swap(S.w_out, S.w_bout);
+    std::swap(S.w_tokoff, S.w_bbase);
+    memcpy(S.last_ms, ms1, sizeof(ms1));
+    S.last_ms[4] += ms2;                  // device time of the chunk: run 1, then scan + gather + run 2
+    S.last_launches = launches1 + launches2 + 9;
+    return B200BPE_OK;
+}
+
 // --------------------------------------------------------------------------------------------
 // host path: host buffers in, ONE pinned result out; chunks round-robin over the devices
 // --------------------------------------------------------------------------------------------
 struct HostJob {
     b200bpe *h = nullptr;
     const uint8_t *text = nullptr; const uint64_t *doc_off = nullptr; uint64_t n_docs = 0;
-    bool single_piece = false, pageable = false;
+    bool single_piece = false, pageable = false, bytes = false;
     const uint8_t *sp_flags = nullptr;
     std::vector<uint64_t> cut;                    // chunk c = documents [cut[c], cut[c+1])
     std::vector<std::atomic<long long>> count;    // tokens of chunk c, -1 until its kernels are done
@@ -942,6 +1060,7 @@ struct HostJob {
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; std::mutex stat_mu;
     uint32_t grown = 0, reruns = 0;               // B200BPE_GREW_* bits / pipeline re-runs of all workers (under stat_mu)
     uint64_t cls[N_CLS] = {};                     // long pieces per length class of the chunks' final runs (under stat_mu)
+    uint64_t bytes_repairs = 0;                   // bytes mode: documents repaired (under stat_mu)
 
     void set_error(int rc) {
         std::lock_guard<std::mutex> lk(err_mu);
@@ -1043,12 +1162,13 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         PipeArgs a;
         a.d_text = S.w_text.p; a.n_bytes = doc_off[hi] - doc_off[lo]; a.d_doc_off = S.w_docoff.p; a.n_docs = hi - lo;
         a.d_out = S.w_out.p; a.d_tok_off = S.w_tokoff.p; a.st = S.stream; a.single_piece = J->single_piece; a.sp_flags = J->sp_flags;
+        a.bytes = J->bytes;
         return a;
     };
     size_t known = 0; uint64_t known_sum = 0;                    // prefix of the per-chunk token counts seen so far
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; float last_d2h = 0;
     uint32_t grown = 0, reruns = 0;
-    uint64_t cls[N_CLS] = {};
+    uint64_t cls[N_CLS] = {}, repaired = 0;
     // finalise chunk k: wait for its kernels, then send its offsets + tokens home (async) at their final place
     auto drain = [&](size_t k) -> int {
         Slot &S = slot_of(k);
@@ -1068,8 +1188,13 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         }
         if (rc) return rc;
         float h2d = 0; cudaEventElapsedTime(&h2d, S.ev[5], S.ev[6]);
-        const uint64_t nt = S.h_ctr->total_tokens;
+        uint64_t nt = S.h_ctr->total_tokens;
         for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
+        if (J->bytes && S.h_bytes->n_docs) {                     // documents that are not well-formed UTF-8: run 2 + splice
+            repaired += S.h_bytes->n_docs;
+            rc = bytes_tail_runs(h, D, S, args_of(k), &nt, cls, &grown, &reruns);
+            if (rc) return rc;
+        }
         J->count[c].store((long long)nt);
         while (known < c) {                                      // token base = counts of all earlier chunks (other devices)
             long long v = J->count[known].load();
@@ -1130,10 +1255,11 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     J->launches += launches;
     J->grown |= grown; J->reruns += reruns;
     for (int i = 0; i < N_CLS; i++) J->cls[i] += cls[i];
+    J->bytes_repairs += repaired;
 }
 
 static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, bool single_piece,
-                       const uint8_t *sp_flags, b200bpe_result **out, int *special_idx) {
+                       const uint8_t *sp_flags, b200bpe_result **out, int *special_idx, bool bytes = false) {
     const uint64_t n_bytes = doc_off[n_docs];
     if (doc_off[0] != 0) return fail(B200BPE_EINVAL, "document offsets must start at 0");
     const int n_dev = (int)h->devs.size();
@@ -1171,7 +1297,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
     for (int pass = 0; pass < 2; pass++) {
         HostJob J;
         J.h = h; J.text = text; J.doc_off = doc_off; J.n_docs = n_docs; J.single_piece = single_piece; J.pageable = pageable;
-        J.sp_flags = sp_flags; J.cut = cut;
+        J.sp_flags = sp_flags; J.cut = cut; J.bytes = bytes;
         J.count = std::vector<std::atomic<long long>>(n_chunks);
         for (auto &c : J.count) c.store(-1);
         b200bpe_result *r = new b200bpe_result();
@@ -1201,6 +1327,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
         memcpy(h->last_ms, J.sum_ms, sizeof(J.sum_ms)); h->last_launches = J.launches;
         r->n_tokens = total;
         h->set_piece_classes(J.cls);
+        h->last_bytes_repairs = J.bytes_repairs;
         h->live_results++;                                        // caller holds h->mu
         *out = r;
         return B200BPE_OK;
@@ -1216,6 +1343,21 @@ extern "C" int b200bpe_encode_ordinary_batch(b200bpe_t *h, const uint8_t *text, 
     std::lock_guard<std::mutex> lk(h->mu);
     DeviceGuard guard;
     return encode_host(h, text, doc_off, n_docs, false, nullptr, out, nullptr);
+}
+
+// CoreBPE::_encode_bytes (src/py.rs:72-115) for every document of a batch: documents that are well-formed UTF-8 get
+// exactly the tokens of b200bpe_encode_ordinary_batch; the others are cut at their first ill-formed byte and repaired on
+// the device (kernels_bytes.cuh).
+extern "C" int b200bpe_encode_bytes_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
+                                          b200bpe_result_t **out) {
+    if (h) h->reset_reruns();
+    if (!h || !doc_off || !out) return fail(B200BPE_EINVAL, "null argument");
+    if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
+    if (!h->decode_on_device)
+        return fail(B200BPE_EINVAL, "bytes mode reads token lengths from the device decode tables: every token id must be < 2^24");
+    std::lock_guard<std::mutex> lk(h->mu);
+    DeviceGuard guard;
+    return encode_host(h, text, doc_off, n_docs, false, nullptr, out, nullptr, true);
 }
 
 extern "C" int b200bpe_encode_single_piece(b200bpe_t *h, const uint8_t *piece, uint64_t len, b200bpe_result_t **out) {
@@ -1427,6 +1569,12 @@ extern "C" int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *
     if (!h) return fail(B200BPE_EINVAL, "null handle");
     if (counts8) for (int c = 0; c < N_CLS; c++) counts8[c] = h->last_cls[c].load();
     if (lane_per_piece) *lane_per_piece = h->last_lane_per_piece.load();
+    return B200BPE_OK;
+}
+
+extern "C" int b200bpe_last_bytes_repairs(b200bpe_t *h, uint64_t *n_docs_repaired) {
+    if (!h) return fail(B200BPE_EINVAL, "null handle");
+    if (n_docs_repaired) *n_docs_repaired = h->last_bytes_repairs.load();
     return B200BPE_OK;
 }
 

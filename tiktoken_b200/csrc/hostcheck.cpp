@@ -121,8 +121,9 @@ extern "C" uint32_t hc_probe_long(void *p, const uint8_t *piece, uint32_t len) {
 }
 
 // the bit-parallel span evaluator the pre-tokeniser kernel actually runs (pretok_fast.cuh)
-extern "C" int hc_piece_starts_fast(int pattern, const uint8_t *text, int64_t n, const uint64_t *doc_off,
-                                    int64_t n_docs, uint8_t *is_start /* n+1 bytes */, uint64_t *stats2) {
+template <bool CUT>
+static int piece_starts_fast(int pattern, const uint8_t *text, int64_t n, const uint64_t *doc_off, int64_t n_docs,
+                             uint8_t *is_start, uint64_t *stats2) {
     std::vector<uint8_t> padded((size_t)n + 64, 0);
     memcpy(padded.data(), text, (size_t)n);
     const int64_t n_words = (n + 1 + 31) / 32;
@@ -137,9 +138,9 @@ extern "C" int hc_piece_starts_fast(int pattern, const uint8_t *text, int64_t n,
     SpanStats st{0, 0};
     for (int64_t w = 0; w < n_words; w++) {
         uint32_t word;
-        if (pattern == PAT_R50K) word = span_boundaries<PAT_R50K>(t, w, &st);
-        else if (pattern == PAT_CL100K) word = span_boundaries<PAT_CL100K>(t, w, &st);
-        else if (pattern == PAT_O200K) word = span_boundaries<PAT_O200K>(t, w, &st);
+        if (pattern == PAT_R50K) word = span_boundaries<PAT_R50K, CUT>(t, w, &st);
+        else if (pattern == PAT_CL100K) word = span_boundaries<PAT_CL100K, CUT>(t, w, &st);
+        else if (pattern == PAT_O200K) word = span_boundaries<PAT_O200K, CUT>(t, w, &st);
         else return -1;
         for (int j = 0; j < 32; j++) {
             int64_t pos = w * 32 + j;
@@ -147,5 +148,34 @@ extern "C" int hc_piece_starts_fast(int pattern, const uint8_t *text, int64_t n,
         }
     }
     if (stats2) { stats2[0] = st.positions; stats2[1] = st.slow; }
+    return 0;
+}
+extern "C" int hc_piece_starts_fast(int pattern, const uint8_t *text, int64_t n, const uint64_t *doc_off,
+                                    int64_t n_docs, uint8_t *is_start /* n+1 bytes */, uint64_t *stats2) {
+    return piece_starts_fast<false>(pattern, text, n, doc_off, n_docs, is_start, stats2);
+}
+// the same, as the bytes mode's pre-tokeniser runs it (pretok_kernel<PAT, true>): haystack starts may follow ill-formed leads
+extern "C" int hc_piece_starts_fast_cut(int pattern, const uint8_t *text, int64_t n, const uint64_t *doc_off,
+                                        int64_t n_docs, uint8_t *is_start, uint64_t *stats2) {
+    return piece_starts_fast<true>(pattern, text, n, doc_off, n_docs, is_start, stats2);
+}
+
+// the UTF-8 classifier of the bytes mode (utf8_check.cuh): valid_up_to of every document (its length when well-formed),
+// from the first mark of each document, the way utf8_check_kernel reduces them
+#include "utf8_check.cuh"
+
+extern "C" int hc_utf8_valid_up_to(const uint8_t *text, int64_t n, const uint64_t *doc_off, int64_t n_docs, uint64_t *vup) {
+    const int64_t n_words = (n + 1 + 31) / 32;
+    std::vector<uint32_t> dbits((size_t)n_words + 4, 0);
+    for (int64_t d = 0; d <= n_docs; d++) dbits[doc_off[d] >> 5] |= 1u << (doc_off[d] & 31);
+    for (int64_t d = 0; d < n_docs; d++) vup[d] = doc_off[d + 1] - doc_off[d];
+    int64_t d = 0;
+    for (int64_t w = 0; w < n_words; w++) {
+        for (uint32_t m = utf8_bad_word(text, n, dbits.data(), w); m; m &= m - 1) {
+            const uint64_t pos = (uint64_t)(w * 32 + __builtin_ctz(m));
+            while (doc_off[d + 1] <= pos) d++;
+            if (pos - doc_off[d] < vup[d]) vup[d] = pos - doc_off[d];
+        }
+    }
     return 0;
 }

@@ -53,7 +53,8 @@ __device__ __forceinline__ bool slow_boundary(const TextAccess &t, long long pos
 // Fast part: the bit-parallel rules decide all but a fraction of a percent of the positions (none on English text);
 // the rest go to a global list.  Keeping the general rule function OUT of this kernel keeps its register
 // count low and its warps convergent -- the function is long, branchy and walks along runs.
-template <int PAT>
+// CUT: bytes mode (a haystack may start right after an ill-formed lead byte, see classify_window)
+template <int PAT, bool CUT = false>
 __global__ void __launch_bounds__(PRETOK_WARPS * 32, PAT == PAT_O200K ? 4 : 5) pretok_kernel(const uint8_t *__restrict__ text, long long n_bytes,
                                                                   const uint32_t *__restrict__ dbits, UcTables uc,
                                                                   uint32_t *__restrict__ pbits, uint32_t *__restrict__ psum,
@@ -65,7 +66,7 @@ __global__ void __launch_bounds__(PRETOK_WARPS * 32, PAT == PAT_O200K ? 4 : 5) p
     const TextAccess t{text, n_bytes, dbits, uc.stage1, uc.stage2, uc.ascii, uc.one};
     if (threadIdx.x == 0) s_cnt = 0;
     uint64_t b = 0, slow = 0;
-    if (w < n_words) b = span_fast<PAT>(t, w, slow);
+    if (w < n_words) b = span_fast<PAT, CUT>(t, w, slow);
     uint32_t sm = (uint32_t)(slow >> 8);                // own positions only
     if (ibits && w < n_words) sm &= ~ibits[w];          // inside an accepted special token: no piece start, nothing to decide
     uint32_t word = 0;
@@ -116,16 +117,15 @@ __global__ void __launch_bounds__(256) pretok_slow_kernel(const uint8_t *__restr
     }
 }
 
-// single-piece mode (encode_single_piece): P = {0, n_bytes}
-__global__ void single_piece_bits_kernel(uint32_t *pbits, uint32_t *psum, long long n_bytes, long long n_words) {
+// single-piece mode: every document is one piece, P = D (encode_single_piece is its one-document case; the bytes mode's
+// run 2 encodes the unstable piece of every damaged document this way)
+__global__ void single_piece_bits_kernel(uint32_t *pbits, uint32_t *psum, const uint32_t *__restrict__ dbits, long long n_words) {
     long long w = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     uint32_t word = 0;
     if (w < n_words) {
-        if (w == 0) word |= 1u;
-        if ((n_bytes >> 5) == w) word |= 1u << (n_bytes & 31);
+        word = dbits[w];
         pbits[w] = word;
     }
     const uint32_t nz = __ballot_sync(0xFFFFFFFFu, word != 0);
     if ((threadIdx.x & 31) == 0 && (w >> 5) <= ((n_words - 1) >> 5)) psum[w >> 5] = nz;
 }
-

@@ -101,7 +101,9 @@ struct WinMasks {
     uint64_t LU, LL, LB, M, N, NA, SP, WS, NL, APOS, SLASH, O;   // WS: non-SP non-CR/LF whitespace
 };
 
-// Classify the window [win0, win0+48).  Non-ASCII scalars are decoded one by one.
+// Classify the window [win0, win0+48).  Non-ASCII scalars are decoded one by one.  CUT (bytes mode, where a document
+// may end in an ill-formed lead byte): a lead does not paint its class past the next document or haystack start.
+template <bool CUT = false>
 B2_HD void classify_window(const TextAccess &t, int64_t win0, int64_t w, WinMasks &m) {
     uint32_t W[12];
     const int64_t n = t.n;
@@ -159,6 +161,10 @@ B2_HD void classify_window(const TextAccess &t, int64_t win0, int64_t w, WinMask
         const int c = t.cls(pos);
         uint64_t bits = ((1ull << len) - 1ull) << j;
         bits &= valid;
+        if (CUT) {
+            const uint64_t cross = D & bits & ~(1ull << j);
+            if (cross) bits &= (cross & (0ull - cross)) - 1ull;
+        }
         switch (c) {
             case C_LU: m.LU |= bits; break;
             case C_LL: m.LL |= bits; break;
@@ -174,13 +180,13 @@ B2_HD void classify_window(const TextAccess &t, int64_t win0, int64_t w, WinMask
 // Fast part of a span: returns the boundary bits the local picture decides (window bit i = byte win0 + i,
 // own bytes are bits 8..39; document starts included) and, in `slow_out`, the own positions that
 // must be decided by the general rule function boundary_before<PAT>().
-template <int PAT>
+template <int PAT, bool CUT = false>
 B2_HD uint64_t span_fast(const TextAccess &t, int64_t w, uint64_t &slow_out, SpanStats *stats = nullptr) {
     const int64_t base = w * 32, win0 = base - 8;
     slow_out = 0;
     if (base > t.n) return 0;
     WinMasks m;
-    classify_window(t, win0, w, m);
+    classify_window<CUT>(t, win0, w, m);
     const uint64_t OWN = 0xFFFFFFFFull << 8;
     const uint64_t lead = m.valid & ~m.cont;
     const uint64_t own = OWN & lead & ~m.D;              // positions to decide (doc starts are forced)
@@ -385,10 +391,10 @@ B2_HD uint32_t span_word(const TextAccess &t, int64_t w, uint64_t b) {
 }
 
 // one span, start to finish, by one thread (host checks, and the reference for the kernel's warp-cooperative form)
-template <int PAT>
+template <int PAT, bool CUT = false>
 B2_HD uint32_t span_boundaries(const TextAccess &t, int64_t w, SpanStats *stats = nullptr) {
     uint64_t slow;
-    uint64_t b = span_fast<PAT>(t, w, slow, stats);
+    uint64_t b = span_fast<PAT, CUT>(t, w, slow, stats);
     const int64_t win0 = w * 32 - 8;
     for (uint64_t s = slow; s;) {
         const int j = B2_CTZLL(s); s &= s - 1;
