@@ -181,6 +181,16 @@ int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *lane_per_pi
  * repaired, summed over chunks and devices.  0 after any other encode call and after a call that failed. */
 int b200bpe_last_bytes_repairs(b200bpe_t *h, uint64_t *n_docs_repaired);
 
+/* What the miss memo did in the most recent encode call on this handle, summed over chunks and devices, from the runs
+ * whose output the call returned: *misses = pieces of up to 16 bytes that are not tokens (a single byte only when the
+ * vocabulary lacks it), *merged = those merged (one per distinct piece, plus every piece of 16 bytes and every piece the
+ * memo did not place), *unplaced = pieces of up to 15 bytes the memo did not place: they found neither their key nor an
+ * empty slot within 8 probe steps, or their part of the memo had stopped (full, or too few repeats to pay).  The memo lives for one call; its size is
+ * B200BPE_MISS_MEMO_SLOTS slots (0: off, every miss is merged) or, unset, one slot per 128 bytes of a chunk, from 2^12
+ * to 2^21.  After a queued device series the counts describe its last call.  Reset to zeros where b200bpe_last_reruns
+ * is, and left at zeros by a call that fails. */
+int b200bpe_last_miss_memo(b200bpe_t *h, uint64_t *misses, uint64_t *merged, uint64_t *unplaced);
+
 /* Sizes of the device tables (bytes) for reporting: [0] piece tables (narrow + wide), [1] pair table,
  * [2] long-token table + blob, [3] Unicode class tables. */
 int b200bpe_table_bytes(b200bpe_t *h, uint64_t *bytes4);

@@ -80,6 +80,8 @@ def lib() -> C.CDLL:
     L.b200bpe_encode_bytes_batch.argtypes = [vp, vp, vp, u64, C.POINTER(vp)]
     L.b200bpe_last_bytes_repairs.restype = i32
     L.b200bpe_last_bytes_repairs.argtypes = [vp, C.POINTER(u64)]
+    L.b200bpe_last_miss_memo.restype = i32
+    L.b200bpe_last_miss_memo.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
     L.b200bpe_encode_single_piece.restype = i32
     L.b200bpe_encode_single_piece.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.b200bpe_result_tokens.restype = vp
@@ -119,7 +121,7 @@ EXPORTS = [
     "b200bpe_decode_bytes", "b200bpe_decode_batch", "b200bpe_last_timings", "b200bpe_table_bytes", "b200bpe_last_error",
     "b200bpe_version", "b200bpe_device_count", "b200bpe_create_multi", "b200bpe_n_devices", "b200bpe_encode_batch_special",
     "b200bpe_special_name", "b200bpe_encode_device_async", "b200bpe_device_wait", "b200bpe_trim", "b200bpe_last_reruns",
-    "b200bpe_last_piece_classes", "b200bpe_encode_bytes_batch", "b200bpe_last_bytes_repairs",
+    "b200bpe_last_piece_classes", "b200bpe_encode_bytes_batch", "b200bpe_last_bytes_repairs", "b200bpe_last_miss_memo",
 ]
 
 GREW_MISS, GREW_SLOW, GREW_LONG = 1, 2, 4       # B200BPE_GREW_* (b200bpe_last_reruns)

@@ -390,6 +390,16 @@ class CoreBPE:
         _lib.check(self._L.b200bpe_last_bytes_repairs(self._h, C.byref(n)))
         return int(n.value)
 
+    def last_miss_memo(self) -> dict:
+        """What the per-call miss memo did in the most recent encode call: `misses` = pieces of up to 16 bytes that are
+        not tokens (a single byte only when the vocabulary lacks it), `merged` = those merged (one per distinct piece, plus
+        16-byte and unplaced ones; the others copy their owner's tokens), `unplaced` = pieces the memo did not place (no
+        room, or it had stopped because it was full or did not pay).  Summed over chunks and devices; zeros after a call
+        that failed."""
+        v = [C.c_uint64(0) for _ in range(3)]
+        _lib.check(self._L.b200bpe_last_miss_memo(self._h, *(C.byref(x) for x in v)))
+        return {"misses": int(v[0].value), "merged": int(v[1].value), "unplaced": int(v[2].value)}
+
     def trim(self) -> None:
         """Give the engine's grow-only device work-spaces and pooled pinned blocks back (tables stay)."""
         _lib.check(self._L.b200bpe_trim(self._h))

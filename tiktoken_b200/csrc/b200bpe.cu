@@ -16,8 +16,9 @@
 //                         -- the round-synchronous exact merge in global scratch
 //   probe_kernel          persistent warps, TMA-staged 1 KiB sub-tiles: whole-piece table probe of every short piece
 //                         (one 32 B sector each), one slot per piece, misses -> global queue with their key bytes
-//   miss_{hist,base,scatter}, miss_kernel   the ~5 % misses, sorted by length, one piece per lane,
-//                         warp-convergent exact min-rank merge on dense records
+//   miss_{dedup,base,scatter}, miss_kernel, miss_fanout   the ~5 % misses: one owner per distinct piece (a per-call
+//                         memo), owners sorted by length, one piece per lane, warp-convergent exact min-rank merge on
+//                         dense records, the owner's result copied to every other occurrence
 //   scan_{partial,top,final}, gather_kernel, big_copy_kernel   token counts -> offsets -> tokens and
 //                         per-document offsets at their final place
 //   utf8_check, bytes_*   (bytes mode only, kernels_bytes.cuh) documents that are not well-formed UTF-8: cut at the
@@ -174,6 +175,7 @@ struct Slot {
     DevBuf<uint8_t> w_text; DevBuf<unsigned long long> w_docoff, w_tokoff, w_sub_base;
     DevBuf<uint32_t> w_ptok, w_mres, w_mq_pos, w_mq_roff, w_doc_tiles, w_sub_count; DevBuf<uint8_t> w_mq_len;
     DevBuf<uint4> w_mq_key, w_mq_skey, w_mq_smeta, w_mq_rec;
+    DevBuf<uint4> w_memo_key; DevBuf<uint32_t> w_memo_owner, w_mq_slot, w_mq_own, w_memo_bn;   // miss memo (MissMemo)
     DevBuf<uint32_t> w_dbits, w_pbits, w_psum, w_sfd, w_lidx, w_out, w_ltok, w_hbits, w_ibits, w_sbits, w_cbits, w_slow;
     DevBuf<unsigned long long> w_lq_start, w_lq_off; DevBuf<unsigned int> w_lq_len, w_lq_ntok, w_lq_cls, w_big_n, w_sort_hist;
     DevBuf<unsigned long long> w_big_dst, w_big_src, w_scan_part;
@@ -221,6 +223,7 @@ struct Slot {
         w_text.release(); w_docoff.release(); w_tokoff.release(); w_sub_base.release();
         w_ptok.release(); w_mres.release(); w_mq_pos.release(); w_mq_roff.release(); w_doc_tiles.release(); w_sub_count.release();
         w_mq_len.release(); w_mq_rec.release(); w_mq_key.release(); w_mq_skey.release(); w_mq_smeta.release();
+        w_memo_key.release(); w_memo_owner.release(); w_mq_slot.release(); w_mq_own.release(); w_memo_bn.release();
         w_dbits.release(); w_pbits.release(); w_psum.release(); w_sfd.release(); w_lidx.release(); w_out.release(); w_ltok.release();
         w_hbits.release(); w_ibits.release(); w_sbits.release(); w_cbits.release(); w_slow.release(); w_spflags.release();
         w_lq_start.release(); w_lq_off.release(); w_lq_len.release(); w_lq_ntok.release(); w_lq_cls.release(); w_big_n.release();
@@ -307,8 +310,12 @@ struct b200bpe {
     std::atomic<uint64_t> last_cls[N_CLS] = {};
     std::atomic<int> last_lane_per_piece{0};
     std::atomic<uint64_t> last_bytes_repairs{0};   // documents the most recent bytes-mode call repaired (b200bpe_last_bytes_repairs)
+    // missed pieces, those merged and those the memo could not place, of the runs whose output the most recent encode call
+    // returned (b200bpe_last_miss_memo)
+    std::atomic<uint64_t> last_memo[3] = {};
     void reset_reruns() {
         last_grown = 0; last_reruns = 0; last_token_passes = 0; last_bytes_repairs = 0;
+        for (auto &c : last_memo) c = 0;
         for (auto &c : last_cls) c = 0;
         last_lane_per_piece = 0;
     }
@@ -316,10 +323,12 @@ struct b200bpe {
         for (int c = 0; c < N_CLS; c++) last_cls[c] = cls[c];
         last_lane_per_piece = mid_group ? 0 : 1;
     }
+    void set_miss_memo(const uint64_t *memo) { for (int i = 0; i < 3; i++) last_memo[i] = memo[i]; }
     size_t chunk_bytes = 64u << 20; bool chunk_forced = false;
     int copy_threads = 4;
     TaskPool *pool = nullptr;        // helper threads (created with the first host-path call)
     int pack_bits = 0;               // host path: tokens cross PCIe as fields of this many bits (0: plain u32)
+    long memo_slots = -1;            // miss memo slots per call: -1 from the batch size, 0 off (B200BPE_MISS_MEMO_SLOTS)
     bool mid_group = true;           // 17..1024-byte pieces: group-of-lanes kernels (need ranks < 2^22)
     bool pmerge = true;              // 129..1024-byte pieces: segmented parallel merge (needs ranks < 2^22); off: the group-of-lanes kernels
     int pmerge_min_cls = 3;          // shortest length class the parallel merge takes (3: 129..256 bytes; 0: everything from 17 bytes)
@@ -530,6 +539,7 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
     h->mid_group = H.max_rank < MIDG_MAX_RANK && env_long("B200BPE_MID_GROUP", 1, 0, 1) != 0;
     h->pmerge = h->mid_group && env_long("B200BPE_PMERGE", 1, 0, 1) != 0;
     h->pmerge_min_cls = (int)env_long("B200BPE_PMERGE_MIN_CLS", 3, 1, 3);
+    h->memo_slots = env_long("B200BPE_MISS_MEMO_SLOTS", -1, 0, 1l << 24);
     h->copy_threads = (int)env_long("B200BPE_COPY_THREADS", std::max(1u, std::min(16u, std::thread::hardware_concurrency() / 4)), 1, 64);
     {   // tokens return over PCIe as bit fields just wide enough for the largest id (17 bits for cl100k, 18 for o200k, 16 for
         // r50k / p50k instead of 32): the return traffic shares the link with the text going up
@@ -640,6 +650,17 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         CUDA_TRY(S.w_mq_key.ensure(mcap)); CUDA_TRY(S.w_mq_skey.ensure(mcap)); CUDA_TRY(S.w_mq_smeta.ensure(mcap));
         CUDA_TRY(S.w_mres.ensure(S.mres_cap + 64));
         CUDA_TRY(S.w_sort_hist.ensure((size_t)D->n_sm * SORT_BLOCKS_PER_SM * 17 + 32));
+        CUDA_TRY(S.w_mq_slot.ensure(mcap)); CUDA_TRY(S.w_mq_own.ensure(mcap));
+        CUDA_TRY(S.w_memo_bn.ensure((size_t)D->n_sm * SORT_BLOCKS_PER_SM * 2 + 4));
+    }
+    // miss memo: one slot per 128 bytes of text (a 16-byte key and a u32 owner), from 2^12 to 2^21 slots
+    uint32_t memo_slots = 0;
+    if (h->memo_slots) {
+        const uint64_t want = h->memo_slots > 0 ? (uint64_t)h->memo_slots
+                                                : std::min<uint64_t>(std::max<uint64_t>(n_bytes / 128, 1u << 12), 1u << 21);
+        memo_slots = 1;
+        while (memo_slots < want) memo_slots <<= 1;
+        CUDA_TRY(S.w_memo_key.ensure(memo_slots)); CUDA_TRY(S.w_memo_owner.ensure(memo_slots));
     }
     {   // undecided pre-tokeniser positions: under 2 % on the worst corpus seen; sized for 12 %, grown on ERR_SLOWCAP
         const size_t want = std::max<size_t>((size_t)(n_bytes / 8) + 4096, MISS_CAP_MIN);
@@ -797,15 +818,21 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         p.sub_count = S.w_sub_count.p; p.sub_base = S.w_sub_base.p;
         p.out = a.d_out; p.tok_off = a.d_tok_off; p.ctr = S.d_ctr;
         p.big_dst = S.w_big_dst.p; p.big_src = S.w_big_src.p; p.big_n = S.w_big_n.p;
+        MissMemo memo;
+        memo.key = S.w_memo_key.p; memo.owner = S.w_memo_owner.p; memo.slot = S.w_mq_slot.p; memo.own = S.w_mq_own.p;
+        memo.block_n = S.w_memo_bn.p; memo.mask = memo_slots ? memo_slots - 1 : 0; memo.on = memo_slots ? 1u : 0u;
+        memo.limit = std::max<uint32_t>(1u, memo_slots / 2 / (uint32_t)(D->n_sm * SORT_BLOCKS_PER_SM));   // per dedup block
         const long long want_blocks = (n_tiles + ENC_WARPS - 1) / ENC_WARPS;
         const unsigned probe_grid = (unsigned)std::min<long long>(want_blocks, (long long)D->n_sm * D->probe_blocks_per_sm);
         probe_kernel<<<probe_grid, ENC_WARPS * 32, 0, st>>>(p, D->T);
         CUDA_TRY(cudaEventRecord(S.ev[8], st));
         const int sort_blocks = D->n_sm * SORT_BLOCKS_PER_SM;
-        miss_hist_kernel<<<sort_blocks, 256, 0, st>>>(p, S.w_sort_hist.p);
+        if (memo_slots) CUDA_TRY(cudaMemsetAsync(S.w_memo_key.p, 0, (size_t)memo_slots * sizeof(uint4), st));
+        miss_dedup_kernel<<<sort_blocks, SORT_THREADS, 0, st>>>(p, memo, S.w_sort_hist.p);
         miss_base_kernel<<<1, 17 * 32, 0, st>>>(S.w_sort_hist.p, sort_blocks);
-        miss_scatter_kernel<<<sort_blocks, 256, 0, st>>>(p, S.w_sort_hist.p);
+        miss_scatter_kernel<<<sort_blocks, SORT_THREADS, 0, st>>>(p, memo, S.w_sort_hist.p);
         miss_kernel<<<D->n_sm * 16, MISS_WARPS * 32, 0, st>>>(p, D->T);
+        if (memo_slots) miss_fanout_kernel<<<sort_blocks, SORT_THREADS, 0, st>>>(p, memo);
         CUDA_TRY(cudaEventRecord(S.ev[7], st));
         CUDA_TRY(cudaStreamWaitEvent(st, S.ev[12], 0));          // join: the long pieces' tokens and counts are needed from here on
         CUDA_TRY(cudaStreamWaitEvent(st, S.ev[13], 0));
@@ -829,7 +856,7 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
             launches++;
         }
         finalize_kernel<<<1, 32, 0, st>>>(S.d_ctr, S.d_sticky, a.d_counts, n_docs);
-        launches += sparse_docs ? 12 : 11;
+        launches += (sparse_docs ? 12 : 11) + (memo_slots ? 1 : 0);
     }
     CUDA_TRY(cudaEventRecord(S.ev[4], st));
     if (a.bytes) CUDA_TRY(cudaMemcpyAsync(S.h_bytes, S.d_bytes, sizeof(BytesCounters), cudaMemcpyDeviceToHost, st));
@@ -879,6 +906,11 @@ static int collect_pipeline(b200bpe *h, Slot &S, int *special_idx, uint64_t *spe
     if (c.err & ERR_NOBYTE)
         return fail(B200BPE_ENOBYTE, "a piece needs a single-byte token that mergeable_ranks does not contain");
     return B200BPE_OK;
+}
+
+// what the miss memo did in the pipeline that last ran on S: missed pieces, pieces merged, pieces it could not place
+static void add_miss_memo(const Slot &S, uint64_t *memo) {
+    memo[0] += S.h_ctr->n_miss; memo[1] += S.h_ctr->n_owner; memo[2] += S.h_ctr->n_unplaced;
 }
 
 static int device_args_check(b200bpe *h, const uint8_t *d_text, uint64_t n_bytes, const uint64_t *d_doc_off, uint32_t *d_tokens,
@@ -974,6 +1006,9 @@ extern "C" int b200bpe_device_wait(b200bpe_t *h, uint64_t *n_tokens) {
     uint64_t cls[N_CLS];                  // the last call of a queued series: the counters describe that one
     for (int k = 0; k < N_CLS; k++) cls[k] = S.h_ctr->n_cls[k];
     h->set_piece_classes(cls);
+    uint64_t memo[3] = {};
+    add_miss_memo(S, memo);
+    h->set_miss_memo(memo);
     return B200BPE_OK;
 }
 
@@ -999,8 +1034,8 @@ static void enqueue_scan(const uint32_t *cnt, uint64_t n, unsigned long long *pa
 // minus the last kdrop[d] in front of its run-2 tokens.  The final tokens and offsets end up in S.w_out / S.w_tokoff and
 // *nt is their count.  Run 2 is sized from run 1's counters, which the host already waited for: that is the one extra
 // round trip of a damaged chunk.
-static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, uint64_t *nt, uint64_t *cls, uint32_t *grown,
-                           uint32_t *reruns) {
+static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, uint64_t *nt, uint64_t *cls, uint64_t *memo,
+                           uint32_t *grown, uint32_t *reruns) {
     const uint64_t n1 = S.h_ctr->total_tokens, drop = S.h_bytes->drop;
     const float ms1[9] = {S.last_ms[0], S.last_ms[1], S.last_ms[2], S.last_ms[3], S.last_ms[4], S.last_ms[5], S.last_ms[6],
                           S.last_ms[7], S.last_ms[8]};
@@ -1027,6 +1062,7 @@ static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, u
     if (rc) return rc;
     float ms2 = 0; cudaEventElapsedTime(&ms2, S.ev[15], S.ev[4]);
     for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
+    add_miss_memo(S, memo);
     const uint32_t launches2 = S.last_launches;
     *nt = n1 - drop + S.h_ctr->total_tokens;
     CUDA_TRY(S.w_bout.ensure((size_t)std::max<uint64_t>(*nt, a1.n_bytes) + 64));
@@ -1061,6 +1097,7 @@ struct HostJob {
     uint32_t grown = 0, reruns = 0;               // B200BPE_GREW_* bits / pipeline re-runs of all workers (under stat_mu)
     uint64_t cls[N_CLS] = {};                     // long pieces per length class of the chunks' final runs (under stat_mu)
     uint64_t bytes_repairs = 0;                   // bytes mode: documents repaired (under stat_mu)
+    uint64_t memo[3] = {};                        // miss memo counters of the chunks' final runs (under stat_mu)
 
     void set_error(int rc) {
         std::lock_guard<std::mutex> lk(err_mu);
@@ -1168,7 +1205,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     size_t known = 0; uint64_t known_sum = 0;                    // prefix of the per-chunk token counts seen so far
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; float last_d2h = 0;
     uint32_t grown = 0, reruns = 0;
-    uint64_t cls[N_CLS] = {}, repaired = 0;
+    uint64_t cls[N_CLS] = {}, repaired = 0, memo[3] = {};
     // finalise chunk k: wait for its kernels, then send its offsets + tokens home (async) at their final place
     auto drain = [&](size_t k) -> int {
         Slot &S = slot_of(k);
@@ -1190,9 +1227,10 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         float h2d = 0; cudaEventElapsedTime(&h2d, S.ev[5], S.ev[6]);
         uint64_t nt = S.h_ctr->total_tokens;
         for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
+        add_miss_memo(S, memo);
         if (J->bytes && S.h_bytes->n_docs) {                     // documents that are not well-formed UTF-8: run 2 + splice
             repaired += S.h_bytes->n_docs;
-            rc = bytes_tail_runs(h, D, S, args_of(k), &nt, cls, &grown, &reruns);
+            rc = bytes_tail_runs(h, D, S, args_of(k), &nt, cls, memo, &grown, &reruns);
             if (rc) return rc;
         }
         J->count[c].store((long long)nt);
@@ -1256,6 +1294,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     J->grown |= grown; J->reruns += reruns;
     for (int i = 0; i < N_CLS; i++) J->cls[i] += cls[i];
     J->bytes_repairs += repaired;
+    for (int i = 0; i < 3; i++) J->memo[i] += memo[i];
 }
 
 static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, bool single_piece,
@@ -1328,6 +1367,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
         r->n_tokens = total;
         h->set_piece_classes(J.cls);
         h->last_bytes_repairs = J.bytes_repairs;
+        h->set_miss_memo(J.memo);
         h->live_results++;                                        // caller holds h->mu
         *out = r;
         return B200BPE_OK;
@@ -1569,6 +1609,14 @@ extern "C" int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *
     if (!h) return fail(B200BPE_EINVAL, "null handle");
     if (counts8) for (int c = 0; c < N_CLS; c++) counts8[c] = h->last_cls[c].load();
     if (lane_per_piece) *lane_per_piece = h->last_lane_per_piece.load();
+    return B200BPE_OK;
+}
+
+extern "C" int b200bpe_last_miss_memo(b200bpe_t *h, uint64_t *misses, uint64_t *merged, uint64_t *unplaced) {
+    if (!h) return fail(B200BPE_EINVAL, "null handle");
+    if (misses) *misses = h->last_memo[0].load();
+    if (merged) *merged = h->last_memo[1].load();
+    if (unplaced) *unplaced = h->last_memo[2].load();
     return B200BPE_OK;
 }
 

@@ -97,6 +97,19 @@ B2_HD uint64_t long_hash_word(uint64_t w, uint32_t i) {
 B2_HD uint64_t long_hash_step(uint64_t h, uint64_t w, uint32_t i) { return h ^ long_hash_word(w, i); }
 B2_HD uint64_t long_hash_init(uint64_t len) { return len * 0xC2B2AE3D27D4EB4Full + 0x165667B19E3779F9ull; }
 
+// ---- miss memo key: the zero-padded bytes of a missed piece of 1..15 bytes with its length in byte 15 ------------------
+// Bytes len..14 are zero and byte 15 is the length, so equal keys mean equal (bytes, length), NUL bytes included, and no
+// key is all zero (an empty memo slot).  A 16-byte piece has no spare byte: it is not memoised (false).
+B2_HD bool memo_key(U4 &k, uint32_t len) {
+    if (len >= (uint32_t)SHORT_MAX) return false;
+    k.w |= len << 24;
+    return true;
+}
+B2_HD uint32_t memo_hash(const U4 &k) {
+    const uint64_t lo = ((uint64_t)k.y << 32 | k.x), hi = ((uint64_t)k.w << 32 | k.z);
+    return (uint32_t)(long_hash_word(lo, 0) ^ long_hash_word(hi, 1));
+}
+
 // ---- pair table: linear probing over 16-byte slots {a, b, rank, through} ----------------------------------------
 // `through` is 1 when the probe path of some key passes the slot (bpe_tables.h): a slot that does not hold the key and is
 // not passed through -- an empty slot included -- ends the chain.

@@ -42,6 +42,8 @@ struct Counters {            // device-resident, zeroed per call; copied to pinn
     unsigned int special_idx;        // which disallowed special (ERR_SPECIAL)
     unsigned int ticket;
     unsigned int err;
+    unsigned int n_owner;            // missed pieces that are merged: one per distinct piece, plus the unplaced and 16-byte ones
+    unsigned int n_unplaced;         // missed pieces of <= 15 bytes the miss memo did not place (no key, no empty slot, or memo full)
 };
 
 static const uint32_t GROUP_MAX = 1024;       // pieces up to this length merge in shared memory, a group of lanes per piece
@@ -109,6 +111,26 @@ __device__ __forceinline__ U4 ld_stream_U4(const U4 *p) {
 }
 __device__ __forceinline__ void st_stream_u32(uint32_t *p, uint32_t v) { __stcs(p, v); }
 __device__ __forceinline__ void st_stream_u4(uint4 *p, uint4 v) { __stcs(p, v); }
+
+// ---- 128-bit single-copy-atomic load and compare-and-swap (sm_90: LDG.E.128.STRONG.GPU, ATOMG.E.CAS.128) ----------
+__device__ __forceinline__ uint4 u4_of(unsigned long long lo, unsigned long long hi) {
+    return make_uint4((uint32_t)lo, (uint32_t)(lo >> 32), (uint32_t)hi, (uint32_t)(hi >> 32));
+}
+__device__ __forceinline__ uint4 ld_relaxed_b128(const uint4 *p) {
+    unsigned long long lo, hi;
+    asm volatile("{\n\t.reg .b128 t;\n\tld.relaxed.gpu.global.b128 t, [%2];\n\tmov.b128 {%0, %1}, t;\n\t}"
+                 : "=l"(lo), "=l"(hi) : "l"(p) : "memory");
+    return u4_of(lo, hi);
+}
+// stores v at p if *p == 0; returns the old value (0: stored)
+__device__ __forceinline__ uint4 cas_zero_b128(uint4 *p, uint4 v) {
+    unsigned long long lo, hi;
+    const unsigned long long vlo = (unsigned long long)v.y << 32 | v.x, vhi = (unsigned long long)v.w << 32 | v.z, z = 0;
+    asm volatile("{\n\t.reg .b128 c, v, r;\n\tmov.b128 c, {%2, %2};\n\tmov.b128 v, {%3, %4};\n\t"
+                 "atom.relaxed.gpu.global.cas.b128 r, [%5], c, v;\n\tmov.b128 {%0, %1}, r;\n\t}"
+                 : "=l"(lo), "=l"(hi) : "l"(z), "l"(vlo), "l"(vhi), "l"(p) : "memory");
+    return u4_of(lo, hi);
+}
 
 // ---- mbarrier + TMA 1-D bulk copy (cp.async.bulk, SASS UBLKCP) -------------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }

@@ -68,6 +68,17 @@ extern "C" uint32_t hc_piece_lookup(void *p, const uint8_t *piece, uint32_t len)
     uint64_t k0, k1; pack16(piece, len, k0, k1);
     return piece_lookup16(((HcTables *)p)->H.view(), k0, k1, len);
 }
+// the miss memo's key of a piece of 1..16 bytes, from the zero-padded words the probe kernel queues: 1 and the four key
+// words, or 0 for a piece that is not memoised
+extern "C" int hc_memo_key(const uint8_t *piece, uint32_t len, uint32_t *out4) {
+    if (len == 0 || len > (uint32_t)SHORT_MAX) return -1;
+    uint8_t b[16] = {0};
+    memcpy(b, piece, len);
+    U4 k; memcpy(&k, b, 16);
+    if (!memo_key(k, len)) return 0;
+    memcpy(out4, &k, 16);
+    return 1;
+}
 // slots of the narrow and the wide piece table
 extern "C" void hc_piece_slots(void *p, uint64_t *narrow, uint64_t *wide) {
     const HostTables &H = ((HcTables *)p)->H;

@@ -7,9 +7,11 @@
 //                probes in flight per lane: one 16-byte load per step for a piece of <= 11 bytes, two above.  One 32-bit slot per PIECE goes to `ptok` (token id, or a tagged reference
 //                to the miss queue / the long-piece queue); a miss is appended to a global queue TOGETHER WITH ITS 16
 //                KEY BYTES, so that nothing downstream goes back to the text.
-// miss_*         counting sort of the misses by piece length, carrying the records; miss_kernel: one piece per lane,
-//                32 per warp, all lanes walking one convergent instruction stream (merge_short_conv), the literal
-//                min-rank loop of _byte_pair_merge (src/lib.rs:140-196), reading dense sorted records.
+// miss_*         one owner per distinct missed piece (miss_dedup: a per-call memo), counting sort of the owners by
+//                piece length, carrying the records; miss_kernel: one piece per lane, 32 per warp, all lanes walking
+//                one convergent instruction stream (merge_short_conv), the literal min-rank loop of _byte_pair_merge
+//                (src/lib.rs:140-196), reading dense sorted records; miss_fanout: every other occurrence copies its
+//                owner's result.
 // gather_kernel  one warp per sub-tile, PIECE-parallel: 32 slots per step -> token counts -> warp scan -> tokens and
 //                per-document offsets written at their final position.
 // Kernel boundaries do the ordering; there is no look-back chain and no ticket counter.
@@ -32,6 +34,21 @@ struct MissQ {                // queue of pieces (2..16 bytes) that are not toke
     uint32_t cap;             // capacity of the queue (entries)
     unsigned long long mres_cap;   // capacity of mres (tokens)
 };
+
+// Miss memo of one call: the first occurrence of each distinct missed piece becomes its owner and is the only one merged;
+// the other occurrences copy the owner's result.  Cleared by every call, so a result never depends on an earlier one.
+struct MissMemo {
+    uint4 *key;               // [mask + 1] memo_key of the piece in the slot, 0: empty
+    uint32_t *owner;          // [mask + 1] queue index of the slot's owner
+    uint32_t *slot;           // [queue] memo slot of a duplicate (written for duplicates only)
+    uint32_t *own;            // [queue] per dedup block, in its range of the queue: owners from the front, duplicates from the back
+    uint32_t *block_n;        // [dedup blocks][2] owners and duplicates found by the block
+    uint32_t mask;            // slots - 1 (slots: a power of two)
+    uint32_t limit;           // slots a dedup block may take: half of them, shared out equally
+    uint32_t on;              // 0: every missed piece is its own owner
+};
+static const int MEMO_PROBES = 8;                        // linear probe steps before a piece gives up and owns itself
+static const uint32_t MEMO_TRIAL = 256;                  // slots a dedup block takes before it checks that the memo pays
 
 struct TileParams {
     const uint8_t *text; long long n_bytes; long long n_words; long long n_sub;
@@ -233,23 +250,83 @@ struct MissSmem {
     uint32_t bytes[4 * 32];            // [word][lane]: the piece bytes, little-endian
 };
 
-// counting sort of the miss queue by piece length (so that a warp merges pieces of one length):
-// per-block histograms -> bucket bases -> scatter.  Only block-local shared-memory atomics and
-// 17 values per block in global memory; no hot global counters.
+// Owner election, then a counting sort of the owners by piece length (so that a warp merges pieces of one length):
+// dedup with per-block histograms -> bucket bases -> scatter.  Only block-local shared-memory atomics and 18 values per
+// block in global memory; no hot global counters.
 static const int SORT_BLOCKS_PER_SM = 2;
+static const int SORT_THREADS = 1024;                   // dedup / scatter: few blocks (miss_base walks them serially), many threads
 
 __device__ __forceinline__ uint32_t miss_count(const TileParams &p) { return min(p.ctr->n_miss, p.mq.cap); }
 
-__global__ void __launch_bounds__(256) miss_hist_kernel(TileParams p, unsigned int *block_hist /* [gridDim.x][17] */) {
-    __shared__ unsigned int s_h[17];
+// One missed piece per thread.  A piece looks its key up in the memo (a read first: most keys are there already, and a
+// read does not serialise on a hot slot the way an atomic does), claims an empty slot with a 128-bit CAS, and takes the
+// slot of an equal key as a duplicate.  Winners publish owner[slot]; nobody reads owner[] here, because a duplicate may
+// see the key before its owner has published -- the kernel boundary orders that.  Each block may take an equal share of
+// half the slots, and stops earlier when the memo does not pay: once it has taken MEMO_TRIAL slots and found fewer than
+// one duplicate per 8 slots taken (counted in shared memory, no global counter).  From then on the block's pieces do not read
+// their key or probe at all and own themselves, so text whose misses do not repeat pays little more than the length
+// histogram.  Owners go to the front of the block's range of `own` and their
+// lengths into the block's histogram; duplicates go to the back of the range, for miss_fanout_kernel.
+__global__ void __launch_bounds__(SORT_THREADS) miss_dedup_kernel(TileParams p, MissMemo m, unsigned int *block_hist /* [gridDim.x][17] */) {
+    __shared__ unsigned int s_h[17], s_n, s_d, s_unplaced, s_won;
     if (threadIdx.x < 17) s_h[threadIdx.x] = 0;
+    if (threadIdx.x == 0) { s_n = 0; s_d = 0; s_unplaced = 0; s_won = 0; }
     __syncthreads();
+    const int lane = threadIdx.x & 31;
     const uint32_t n_miss = (p.ctr->err & ERR_MISSCAP) ? 0u : miss_count(p);
     const uint32_t chunk = (n_miss + gridDim.x - 1) / gridDim.x;
     const uint32_t lo = blockIdx.x * chunk, hi = min(n_miss, lo + chunk);
-    for (uint32_t qi = lo + threadIdx.x; qi < hi; qi += 256) atomicAdd(&s_h[p.mq.len[qi]], 1u);
+    const volatile unsigned int *won_so_far = &s_won, *dups_so_far = &s_d;
+    for (uint32_t q0 = lo + (threadIdx.x & ~31u); q0 < hi; q0 += SORT_THREADS) {   // warp-uniform trip count: the ballots below
+        const uint32_t qi = q0 + lane;
+        const bool have = qi < hi;
+        const uint32_t taken = *won_so_far;
+        const bool full = !m.on || taken >= m.limit || (taken >= MEMO_TRIAL && *dups_so_far * 8u < taken);
+        bool dup = false, unplaced = false, won = false;
+        uint32_t len = 0;
+        if (have) {
+            len = p.mq.len[qi];
+            if (m.on && len < (uint32_t)SHORT_MAX) {
+                unplaced = true;
+                if (!full) {
+                    const uint4 raw = ld_stream_u4(p.mq.key + qi);
+                    U4 k{raw.x, raw.y, raw.z, raw.w};
+                    memo_key(k, len);
+                    const uint4 kv = make_uint4(k.x, k.y, k.z, k.w);
+                    const uint32_t h = memo_hash(k);
+                    for (int t = 0; t < MEMO_PROBES; t++) {
+                        const uint32_t j = (h + (uint32_t)t) & m.mask;
+                        uint4 cur = ld_relaxed_b128(m.key + j);
+                        if ((cur.x | cur.y | cur.z | cur.w) == 0u) { cur = cas_zero_b128(m.key + j, kv); won = (cur.x | cur.y | cur.z | cur.w) == 0u; }
+                        if (won) { m.owner[j] = qi; unplaced = false; break; }
+                        if (cur.x == kv.x && cur.y == kv.y && cur.z == kv.z && cur.w == kv.w) { m.slot[qi] = j; dup = true; unplaced = false; break; }
+                    }
+                }
+            }
+        }
+        const bool own = have && !dup;
+        if (own) atomicAdd(&s_h[len], 1u);
+        const uint32_t ob = __ballot_sync(0xFFFFFFFFu, own), db = __ballot_sync(0xFFFFFFFFu, dup);
+        const uint32_t ub = __ballot_sync(0xFFFFFFFFu, unplaced), wb = __ballot_sync(0xFFFFFFFFu, won);
+        uint32_t bo = 0, bd = 0;
+        if (lane == 0) {
+            if (ob) bo = atomicAdd(&s_n, (unsigned)__popc(ob));
+            if (db) bd = atomicAdd(&s_d, (unsigned)__popc(db));
+            if (ub) atomicAdd(&s_unplaced, (unsigned)__popc(ub));
+            if (wb) atomicAdd(&s_won, (unsigned)__popc(wb));
+        }
+        bo = __shfl_sync(0xFFFFFFFFu, bo, 0); bd = __shfl_sync(0xFFFFFFFFu, bd, 0);
+        const uint32_t below = (1u << lane) - 1u;
+        if (own) m.own[lo + bo + __popc(ob & below)] = qi;
+        if (dup) m.own[hi - 1 - (bd + __popc(db & below))] = qi;   // owners + duplicates = hi - lo: the two ends never meet
+    }
     __syncthreads();
     if (threadIdx.x < 17) block_hist[blockIdx.x * 17 + threadIdx.x] = s_h[threadIdx.x];
+    if (threadIdx.x == 0) {
+        m.block_n[2 * blockIdx.x] = s_n; m.block_n[2 * blockIdx.x + 1] = s_d;
+        if (s_n) atomicAdd(&p.ctr->n_owner, s_n);
+        if (s_unplaced) atomicAdd(&p.ctr->n_unplaced, s_unplaced);
+    }
 }
 
 // bucket bases: warp l turns column l of block_hist into exclusive offsets (bucket-major, then block order)
@@ -271,14 +348,15 @@ __global__ void __launch_bounds__(17 * 32) miss_base_kernel(unsigned int *block_
     for (int b = lane; b < n_blocks; b += 32) block_hist[b * 17 + l] += base;
 }
 
-__global__ void __launch_bounds__(256) miss_scatter_kernel(TileParams p, const unsigned int *block_base) {
+__global__ void __launch_bounds__(SORT_THREADS) miss_scatter_kernel(TileParams p, MissMemo m, const unsigned int *block_base) {
     __shared__ unsigned int s_b[17];
     if (threadIdx.x < 17) s_b[threadIdx.x] = block_base[blockIdx.x * 17 + threadIdx.x];
     __syncthreads();
     const uint32_t n_miss = (p.ctr->err & ERR_MISSCAP) ? 0u : miss_count(p);
     const uint32_t chunk = (n_miss + gridDim.x - 1) / gridDim.x;
-    const uint32_t lo = blockIdx.x * chunk, hi = min(n_miss, lo + chunk);
-    for (uint32_t qi = lo + threadIdx.x; qi < hi; qi += 256) {
+    const uint32_t lo = blockIdx.x * chunk, n_own = m.block_n[2 * blockIdx.x];   // the dedup block of the same range
+    for (uint32_t k = threadIdx.x; k < n_own; k += SORT_THREADS) {
+        const uint32_t qi = m.own[lo + k];
         const uint32_t len = p.mq.len[qi];
         const uint32_t s = atomicAdd(&s_b[len], 1u);
         p.mq.skey[s] = ld_stream_u4(p.mq.key + qi);
@@ -290,7 +368,7 @@ __global__ void __launch_bounds__(MISS_WARPS * 32, MISS_MIN_BLOCKS) miss_kernel(
     __shared__ MissSmem smem[MISS_WARPS];
     MissSmem &S = smem[threadIdx.x >> 5];
     const int lane = threadIdx.x & 31;
-    const uint32_t n_miss = (p.ctr->err & ERR_MISSCAP) ? 0u : miss_count(p);
+    const uint32_t n_miss = (p.ctr->err & ERR_MISSCAP) ? 0u : p.ctr->n_owner;   // the sorted owners
     const uint32_t stride = gridDim.x * MISS_WARPS * 32;
     for (uint32_t q0 = (blockIdx.x * MISS_WARPS + (threadIdx.x >> 5)) * 32; q0 < n_miss; q0 += stride) {
         const bool have = q0 + lane < n_miss;
@@ -321,6 +399,32 @@ __global__ void __launch_bounds__(MISS_WARPS * 32, MISS_MIN_BLOCKS) miss_kernel(
             atomicAdd(&p.sub_count[meta.z >> 10], c);
         }
         __syncwarp();
+    }
+}
+
+// One duplicate per thread, from the back of its dedup block's range of `own` (same grid): it takes its owner's record
+// and result region and credits the tokens to its sub-tile (one atomic per run of lanes in the same sub-tile: the probe
+// queues a sub-tile's misses back to back).  Owners credited theirs in miss_kernel.
+__global__ void __launch_bounds__(SORT_THREADS) miss_fanout_kernel(TileParams p, MissMemo m) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t n_miss = (p.ctr->err & ERR_MISSCAP) ? 0u : miss_count(p);
+    const uint32_t chunk = (n_miss + gridDim.x - 1) / gridDim.x;
+    const uint32_t hi = min(n_miss, blockIdx.x * chunk + chunk), n_dup = m.block_n[2 * blockIdx.x + 1];
+    for (uint32_t k0 = threadIdx.x & ~31u; k0 < n_dup; k0 += SORT_THREADS) {   // warp-uniform: the match below
+        const uint32_t k = k0 + lane;
+        uint32_t c = 0, sub = 0xFFFFFFFFu;
+        if (k < n_dup) {
+            const uint32_t qi = m.own[hi - 1 - k];
+            const uint32_t o = m.owner[m.slot[qi]];
+            const uint4 r = p.mq.rec[o];
+            p.mq.rec[qi] = r;
+            if (r.x > 3) p.mq.roff[qi] = p.mq.roff[o];
+            c = r.x;
+            sub = p.mq.pos[qi] >> 10;
+        }
+        const uint32_t same = __match_any_sync(0xFFFFFFFFu, sub);
+        const uint32_t sum = __reduce_add_sync(same, c);
+        if (sub != 0xFFFFFFFFu && lane == __ffs(same) - 1 && sum) atomicAdd(&p.sub_count[sub], sum);
     }
 }
 
