@@ -104,6 +104,26 @@ int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, const uint64
 int b200bpe_encode_bytes_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                b200bpe_result_t **out);
 
+/* Encoding.encode_with_unstable (tiktoken/core.py:208-243 -> src/py.rs:117-131 -> CoreBPE::_encode_unstable_native,
+ * src/lib.rs:483-599) for every document of a batch, with the flags and the disallowed check of
+ * b200bpe_encode_batch_special (B200BPE_ESPECIAL, *special_index = the leftmost offender).  Per document: the tokens of
+ * CoreBPE::encode (lib.rs:375-442) minus those of the last regex piece of its final haystack (none when the document is
+ * empty or ends with an allowed special, lib.rs:430-433), extended backwards over all-space mergeable tokens
+ * (lib.rs:444-481) -- the stable tokens, in *stable like b200bpe_encode_batch_special's result --, and the completions of
+ * the unstable bytes U they covered: (a) every token that starts with U (lib.rs:537-549); (b) for i = 1 .. |U|-1 and every
+ * token t that starts with U[i:], encode_ordinary(U[:i] + t) when that is UTF-8, else byte_pair_encode of it, cut after the
+ * first token at which the byte count reaches |U| (lib.rs:551-584); (c) when |U| > 1 and U ends in a White_Space scalar
+ * after other bytes, byte_pair_encode(front) + byte_pair_encode(last scalar) (lib.rs:586-596).  Each distinct completion
+ * of a document comes once, at its first position in that order (the reference returns a HashSet).
+ * *completions: b200bpe_result_tokens = every completion's tokens back to back, b200bpe_result_offsets = their
+ * boundaries (b200bpe_result_n_docs() + 1 of them), b200bpe_result_groups = per input document the range of its
+ * completions (n_docs + 1).  A missing single-byte token fails with B200BPE_ENOBYTE; every token id must be < 2^24
+ * (the device decode tables give the token bytes), else B200BPE_EINVAL.  Candidate text goes through the encoder in
+ * rounds of at most one chunk (B200BPE_CHUNK_MB). */
+int b200bpe_encode_with_unstable_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
+                                       const uint8_t *flags, b200bpe_result_t **stable, b200bpe_result_t **completions,
+                                       int32_t *special_index);
+
 /* Name of special token `index` (as given to b200bpe_create), or NULL. */
 const char *b200bpe_special_name(b200bpe_t *h, int32_t index);
 
@@ -135,6 +155,9 @@ int b200bpe_encode_single_piece(b200bpe_t *h, const uint8_t *piece, uint64_t len
 const uint32_t *b200bpe_result_tokens(const b200bpe_result_t *r);
 const uint64_t *b200bpe_result_offsets(const b200bpe_result_t *r);
 uint64_t b200bpe_result_n_tokens(const b200bpe_result_t *r);
+/* The completions result of b200bpe_encode_with_unstable_batch: per input document d, its completions are
+ * [groups[d], groups[d+1]); *n_groups = the number of input documents.  NULL (and 0) for every other result. */
+const uint64_t *b200bpe_result_groups(const b200bpe_result_t *r, uint64_t *n_groups);
 uint64_t b200bpe_result_n_docs(const b200bpe_result_t *r);
 void b200bpe_result_free(b200bpe_result_t *r);
 
@@ -180,6 +203,12 @@ int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *lane_per_pi
 /* Documents the most recent b200bpe_encode_bytes_batch call on this handle found not to be well-formed UTF-8 and
  * repaired, summed over chunks and devices.  0 after any other encode call and after a call that failed. */
 int b200bpe_last_bytes_repairs(b200bpe_t *h, uint64_t *n_docs_repaired);
+
+/* What the most recent b200bpe_encode_with_unstable_batch call on this handle did, summed over chunks and devices:
+ * [0] documents with unstable bytes, [1] completion candidates encoded (run 2), [2] of those, the ones that took
+ * byte_pair_encode (single-piece mode: not UTF-8, or the whitespace split), [3] candidate rounds, [4] completions
+ * returned.  Reset to zeros where b200bpe_last_reruns is, and left at zeros by a call that fails. */
+int b200bpe_last_unstable(b200bpe_t *h, uint64_t *stats5);
 
 /* What the miss memo did in the most recent encode call on this handle, summed over chunks and devices, from the runs
  * whose output the call returned: *misses = pieces of up to 16 bytes that are not tokens (a single byte only when the

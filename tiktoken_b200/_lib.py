@@ -15,7 +15,7 @@ import subprocess
 _CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 _SO = os.path.join(_CSRC, "libb200bpe.so")
 _SOURCES = ["b200bpe.cu", "dev_common.cuh", "kernels_pretok.cuh", "kernels_long.cuh", "kernels_mid.cuh", "kernels_pmerge.cuh", "kernels_encode.cuh",
-            "kernels_special.cuh", "kernels_decode.cuh", "kernels_bytes.cuh", "utf8_check.cuh", "bpe_device.cuh", "bpe_tables.h", "pretok_rules.cuh",
+            "kernels_special.cuh", "kernels_decode.cuh", "kernels_bytes.cuh", "kernels_unstable.cuh", "utf8_check.cuh", "bpe_device.cuh", "bpe_tables.h", "pretok_rules.cuh",
             "pretok_fast.cuh", "text_access.cuh", "unicode_classes.inc"]
 
 OK, EINVAL, EPATTERN, EDUPRANK, ECUDA, ENOBYTE, EKEY, ESPECIAL, ECAPACITY = 0, -1, -2, -3, -4, -5, -6, -7, -8
@@ -80,6 +80,12 @@ def lib() -> C.CDLL:
     L.b200bpe_encode_bytes_batch.argtypes = [vp, vp, vp, u64, C.POINTER(vp)]
     L.b200bpe_last_bytes_repairs.restype = i32
     L.b200bpe_last_bytes_repairs.argtypes = [vp, C.POINTER(u64)]
+    L.b200bpe_encode_with_unstable_batch.restype = i32
+    L.b200bpe_encode_with_unstable_batch.argtypes = [vp, vp, vp, u64, vp, C.POINTER(vp), C.POINTER(vp), C.POINTER(C.c_int32)]
+    L.b200bpe_result_groups.restype = vp
+    L.b200bpe_result_groups.argtypes = [vp, C.POINTER(u64)]
+    L.b200bpe_last_unstable.restype = i32
+    L.b200bpe_last_unstable.argtypes = [vp, vp]
     L.b200bpe_last_miss_memo.restype = i32
     L.b200bpe_last_miss_memo.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
     L.b200bpe_encode_single_piece.restype = i32
@@ -122,6 +128,7 @@ EXPORTS = [
     "b200bpe_version", "b200bpe_device_count", "b200bpe_create_multi", "b200bpe_n_devices", "b200bpe_encode_batch_special",
     "b200bpe_special_name", "b200bpe_encode_device_async", "b200bpe_device_wait", "b200bpe_trim", "b200bpe_last_reruns",
     "b200bpe_last_piece_classes", "b200bpe_encode_bytes_batch", "b200bpe_last_bytes_repairs", "b200bpe_last_miss_memo",
+    "b200bpe_encode_with_unstable_batch", "b200bpe_result_groups", "b200bpe_last_unstable",
 ]
 
 GREW_MISS, GREW_SLOW, GREW_LONG = 1, 2, 4       # B200BPE_GREW_* (b200bpe_last_reruns)

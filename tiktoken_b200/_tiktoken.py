@@ -83,6 +83,19 @@ class TokenBuffer:
         self.close()
 
 
+class CompletionBuffer(TokenBuffer):
+    """The completions of `encode_with_unstable_batch_buffer`: `tokens()` holds every completion's tokens back to back,
+    `offsets()` their boundaries (`n_docs` is the number of completions), `groups()` per input document the range of
+    its completions (uint64[n_inputs + 1])."""
+
+    def groups(self) -> np.ndarray:
+        if not self._h:
+            raise ValueError("CompletionBuffer is closed")
+        n = C.c_uint64(0)
+        p = self._L.b200bpe_result_groups(self._h, C.byref(n))
+        return np.asarray(_NativeView(self, int(p), int(n.value) + 1, "<u8"))
+
+
 class DisallowedSpecial(ValueError):
     """The text contains a special token that the call disallows; `.token` names it.  The host class turns it into
     the reference's message (tiktoken/core.py:431-438)."""
@@ -180,12 +193,7 @@ class CoreBPE:
         """CoreBPE::encode for a batch (lib.rs:375-442) plus, when `disallowed_special` is given, the check that
         `Encoding.encode` runs first (core.py:120-124) -- one device scan for both.  Raises the reference's
         ValueError (through `disallowed_error`) naming the leftmost disallowed special."""
-        flags = np.zeros(len(self._special_names) + 1, np.uint8)
-        for i, s in enumerate(self._special_names):
-            if s in allowed_special:
-                flags[i] = 1
-            elif s in disallowed_special:
-                flags[i] = 2
+        flags = self._special_flags(allowed_special, disallowed_special)
         res = C.c_void_p()
         bad = C.c_int32(-1)
         rc = self._L.b200bpe_encode_batch_special(self._h, _ptr(text), _ptr(doc_off), len(doc_off) - 1, _ptr(flags),
@@ -194,6 +202,40 @@ class CoreBPE:
             raise DisallowedSpecial(self._special_names[bad.value])
         _lib.check(rc)
         return TokenBuffer(self._L, res, self)
+
+    def _special_flags(self, allowed_special, disallowed_special) -> np.ndarray:
+        flags = np.zeros(len(self._special_names) + 1, np.uint8)
+        for i, s in enumerate(self._special_names):
+            if s in allowed_special:
+                flags[i] = 1
+            elif s in disallowed_special:
+                flags[i] = 2
+        return flags
+
+    def encode_with_unstable_batch_buffer(self, text: np.ndarray, doc_off: np.ndarray, allowed_special,
+                                          disallowed_special=()) -> tuple[TokenBuffer, CompletionBuffer]:
+        """CoreBPE::_encode_unstable_native (lib.rs:483-599) for every document, with the disallowed check of
+        encode_batch_buffer: (stable tokens, completions).  Each distinct completion of a document comes once, at its
+        first position in the reference's enumeration order."""
+        flags = self._special_flags(allowed_special, disallowed_special)
+        stable, comp = C.c_void_p(), C.c_void_p()
+        bad = C.c_int32(-1)
+        rc = self._L.b200bpe_encode_with_unstable_batch(self._h, _ptr(text if len(text) else np.zeros(1, np.uint8)),
+                                                        _ptr(doc_off), len(doc_off) - 1, _ptr(flags), C.byref(stable),
+                                                        C.byref(comp), C.byref(bad))
+        if rc == _lib.ESPECIAL:
+            raise DisallowedSpecial(self._special_names[bad.value])
+        _lib.check(rc)
+        return TokenBuffer(self._L, stable, self), CompletionBuffer(self._L, comp, self)
+
+    def encode_with_unstable_batch(self, texts: list[str], allowed_special, disallowed_special=()):
+        """-> [(stable tokens, [completion, ...]), ...]; UnicodeEncodeError on lone surrogates (py.rs:120 takes &str)."""
+        text, off = self._pack(texts)
+        sbuf, cbuf = self.encode_with_unstable_batch_buffer(text, off, allowed_special, disallowed_special)
+        grp = cbuf.groups().tolist()
+        stable = self._unpack(sbuf)
+        comps = self._unpack(cbuf)
+        return [(stable[d], comps[grp[d]:grp[d + 1]]) for d in range(len(stable))]
 
     def encode_bytes_batch_buffer(self, text: np.ndarray, doc_off: np.ndarray) -> TokenBuffer:
         """CoreBPE::_encode_bytes (src/py.rs:72-115) for every document: text uint8[N] need not be UTF-8, doc_off
@@ -389,6 +431,13 @@ class CoreBPE:
         n = C.c_uint64(0)
         _lib.check(self._L.b200bpe_last_bytes_repairs(self._h, C.byref(n)))
         return int(n.value)
+
+    def last_unstable(self) -> dict:
+        """What the most recent encode_with_unstable_batch* call did: documents with unstable bytes, candidates encoded,
+        candidates that took byte_pair_encode, candidate rounds and completions returned (zeros after any other call)."""
+        v = (C.c_uint64 * 5)()
+        _lib.check(self._L.b200bpe_last_unstable(self._h, v))
+        return dict(zip(["docs", "encoded", "bpe_candidates", "rounds", "completions"], (int(x) for x in v)))
 
     def last_miss_memo(self) -> dict:
         """What the per-call miss memo did in the most recent encode call: `misses` = pieces of up to 16 bytes that are

@@ -186,6 +186,37 @@ class Encoding(_ref_core.Encoding):
         return self._core_bpe.encode_bytes_batch_buffer(np.ascontiguousarray(data, np.uint8),
                                                         np.ascontiguousarray(doc_off, np.uint64))
 
+    def encode_with_unstable_batch(self, text: Sequence[str], *,
+                                   allowed_special: Literal["all"] | AbstractSet[str] = set(),  # noqa: B006
+                                   disallowed_special: Literal["all"] | Collection[str] = "all",
+                                   num_threads: int = 8) -> list[tuple[list[int], list[list[int]]]]:
+        """`encode_with_unstable` (core.py:208-243) of every text, in one native call: (stable tokens, completions) per
+        text.  Each distinct completion comes once, at its first position in the reference's enumeration order (the
+        reference returns them in hash-set order).  Lone surrogates raise UnicodeEncodeError, as the reference's
+        `encode_with_unstable` does."""
+        allowed_special, disallowed_special = self._policy(allowed_special, disallowed_special)
+        try:
+            return self._core_bpe.encode_with_unstable_batch(list(text), allowed_special, disallowed_special or ())
+        except _tiktoken.DisallowedSpecial as e:
+            _ref_core.raise_disallowed_special_token(e.token)
+
+    def encode_with_unstable_packed(self, text_bytes: np.ndarray, doc_off: np.ndarray, *,
+                                    allowed_special: Literal["all"] | AbstractSet[str] = set(),  # noqa: B006
+                                    disallowed_special: Literal["all"] | Collection[str] = "all"):
+        """`encode_with_unstable_batch` on packed UTF-8 (uint8[N] + uint64[n_docs+1]) -> (stable tokens uint32[T],
+        stable offsets uint64[n_docs+1], completion tokens uint32[K], completion offsets uint64[n_completions+1],
+        groups uint64[n_docs+1]); document d's completions are numbers groups[d] .. groups[d+1]-1."""
+        allowed_special, disallowed_special = self._policy(allowed_special, disallowed_special)
+        try:
+            sbuf, cbuf = self._core_bpe.encode_with_unstable_batch_buffer(
+                np.ascontiguousarray(text_bytes, np.uint8), np.ascontiguousarray(doc_off, np.uint64), allowed_special,
+                disallowed_special or ())
+        except _tiktoken.DisallowedSpecial as e:
+            _ref_core.raise_disallowed_special_token(e.token)
+        with sbuf, cbuf:
+            return (np.array(sbuf.tokens()), np.array(sbuf.offsets()), np.array(cbuf.tokens()), np.array(cbuf.offsets()),
+                    np.array(cbuf.groups()))
+
     # ---------------------------------------------------------------- batch decode: one native call
     def decode_batch(self, batch: Sequence[Sequence[int]], *, errors: str = "replace", num_threads: int = 8) -> list[str]:
         return [b.decode("utf-8", errors=errors) for b in self._core_bpe.decode_bytes_batch(batch)]

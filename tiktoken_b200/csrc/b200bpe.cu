@@ -23,6 +23,8 @@
 //                         per-document offsets at their final place
 //   utf8_check, bytes_*   (bytes mode only, kernels_bytes.cuh) documents that are not well-formed UTF-8: cut at the
 //                         first ill-formed byte, repair of the last piece, a second run over the unstable pieces, splice
+//   unstable_*            (completion search only, kernels_unstable.cuh) the unstable tail of every document, the tokens
+//                         that could continue it, run 2 over the candidates in rounds, truncation and deduplication
 //
 // No tensor cores: nothing here is a contraction.  The work is byte/integer, bound by HBM reads
 // of the text, L2 probes of the rank tables and instruction issue.
@@ -57,6 +59,7 @@
 #include "kernels_special.cuh"
 #include "kernels_decode.cuh"
 #include "kernels_bytes.cuh"
+#include "kernels_unstable.cuh"
 #include "unicode_classes.inc"
 
 using namespace b2bpe;
@@ -186,6 +189,8 @@ struct Slot {
     DevBuf<unsigned long long> w_b2doc, w_b2off, w_bbase, w_bpart;
     // allocated by the first bytes-mode call: the splice's scan (run 2 reuses d_ctr), the repair's counters (h_bytes pinned)
     Counters *d_bctr = nullptr; BytesCounters *d_bytes = nullptr, *h_bytes = nullptr;
+    // completion search: run 1's unstable tail per document (|U|, search items; tokens to drop in w_kdrop)
+    DevBuf<uint32_t> w_ulen, w_unit;
     size_t long_cap = 0;            // entries of the global merge scratch (pieces > 256 bytes), grown on ERR_LONGCAP
     size_t miss_cap = 0, mres_cap = 0;   // miss queue entries / miss result tokens, grown on ERR_MISSCAP
     size_t slow_cap = 0;            // positions left to the general pre-tokeniser rule function, grown on ERR_SLOWCAP
@@ -232,6 +237,7 @@ struct Slot {
         w_flag.release(); w_pack.release();
         w_vup.release(); w_kdrop.release(); w_btail.release(); w_b2out.release(); w_bout.release(); w_btext.release();
         w_b2doc.release(); w_b2off.release(); w_bbase.release(); w_bpart.release();
+        w_ulen.release(); w_unit.release();
         if (stage.p) cudaFreeHost(stage.p);
         stage.p = nullptr; stage.cap = 0;
         if (stage_out.p) cudaFreeHost(stage_out.p);
@@ -254,6 +260,28 @@ struct Slot {
     }
 };
 
+// Completion search work-space of one device (kernels_unstable.cuh): a device searches one chunk at a time.  The search
+// items and the per-round arrays are bounded by a chunk (the round's candidate count and text); only the result (the
+// distinct completions) and the deduplication table grow with what the batch returns.
+struct UnstWs {
+    DevBuf<uint32_t> it_lo, it_cnt, it_bytes, it_doc; DevBuf<unsigned long long> item_base, cbase, tbase, part;
+    DevBuf<uint4> cinfo; DevBuf<uint32_t> o_len, s_len, out_o, out_s, nkeep, slot, keep, kc;
+    DevBuf<unsigned long long> o_off, s_off, tokoff_o, tokoff_s, rcb, rtb, zeros, grp_off;
+    DevBuf<uint8_t> text_o, text_s;
+    DevBuf<unsigned long long> tkey; DevBuf<uint32_t> tidx, tloc;
+    uint32_t tslots_min = 0;                 // grown when a table ran out of slots
+    DevBuf<uint32_t> res_tok, res_doc, grp; DevBuf<unsigned long long> res_off;
+    UnstCounters *d_uc = nullptr, *h_uc = nullptr;   // h_uc pinned
+    Counters *d_sctr = nullptr;              // the scans' total
+    void release() {
+        it_lo.release(); it_cnt.release(); it_bytes.release(); it_doc.release(); item_base.release(); cbase.release();
+        tbase.release(); part.release(); cinfo.release(); o_len.release(); s_len.release(); out_o.release(); out_s.release();
+        nkeep.release(); slot.release(); keep.release(); kc.release(); o_off.release(); s_off.release(); tokoff_o.release();
+        tokoff_s.release(); rcb.release(); rtb.release(); zeros.release(); grp_off.release(); text_o.release(); text_s.release();
+        tkey.release(); tidx.release(); tloc.release(); res_tok.release(); res_doc.release(); grp.release(); res_off.release();
+    }
+};
+
 #ifndef B2_N_SLOTS
 #define B2_N_SLOTS 3          // pipeline slots per device: uploads run B2_N_SLOTS - 2 chunks ahead of the kernels
 #endif
@@ -267,6 +295,9 @@ struct DevCtx {
                                                                        // the first bytes-mode call)
     SpecialTables sp;                                                  // device copy of the special-token patterns
     uint8_t *d_sp_arena = nullptr;
+    UnstTables ut;                                                     // completion search tables (the first such call)
+    uint8_t *d_ut_arena = nullptr;
+    UnstWs uw;                                                         // completion search work-space (one chunk at a time)
     static const int N_SLOTS = B2_N_SLOTS;
     Slot slots[B2_N_SLOTS];
     size_t l2_window = 0; float l2_ratio = 0.f;
@@ -279,6 +310,7 @@ struct b200bpe_result {
     PinnedBuf tok, off;                 // pinned when produced by the engine
     std::vector<uint32_t> vtok;         // used when the result is assembled on the host (fallback special path)
     std::vector<uint64_t> voff;
+    std::vector<uint64_t> vgrp;         // completions of b200bpe_encode_with_unstable_batch: per input document, its range
     bool on_host_vec = false;
     uint64_t n_tokens = 0, n_docs = 0;
 };
@@ -310,11 +342,21 @@ struct b200bpe {
     std::atomic<uint64_t> last_cls[N_CLS] = {};
     std::atomic<int> last_lane_per_piece{0};
     std::atomic<uint64_t> last_bytes_repairs{0};   // documents the most recent bytes-mode call repaired (b200bpe_last_bytes_repairs)
+    std::atomic<uint64_t> last_unstable[5] = {};   // b200bpe_last_unstable
+    // completion search tables on the host, built by the first b200bpe_encode_with_unstable_batch call (then uploaded to
+    // every device): mergeable ids in byte order, prefix sums of their lengths, all-space bits of the mergeable tokens,
+    // per-id UTF-8 facts, and the byte_pair_encode of every token its own merges do not reach
+    struct {
+        bool built = false;
+        std::vector<uint32_t> sorted, space, ur_idx, ur_off, ur_tok; std::vector<unsigned long long> lenpre;
+        std::vector<uint8_t> u8info; uint32_t max_len = 0;
+    } uh;
     // missed pieces, those merged and those the memo could not place, of the runs whose output the most recent encode call
     // returned (b200bpe_last_miss_memo)
     std::atomic<uint64_t> last_memo[3] = {};
     void reset_reruns() {
         last_grown = 0; last_reruns = 0; last_token_passes = 0; last_bytes_repairs = 0;
+        for (auto &c : last_unstable) c = 0;
         for (auto &c : last_memo) c = 0;
         for (auto &c : last_cls) c = 0;
         last_lane_per_piece = 0;
@@ -381,6 +423,8 @@ static void devctx_destroy(DevCtx *D) {
     if (D->d_tok_blob) cudaFree(D->d_tok_blob);
     if (D->d_tok_space) cudaFree(D->d_tok_space);
     if (D->d_sp_arena) cudaFree(D->d_sp_arena);
+    if (D->d_ut_arena) cudaFree(D->d_ut_arena);
+    D->uw.release();
     delete D;
 }
 
@@ -619,6 +663,7 @@ struct PipeArgs {
     cudaStream_t st = nullptr;
     bool single_piece = false;                   // every document is one piece (P = D)
     bool bytes = false;                          // bytes mode: documents need not be UTF-8 (kernels_bytes.cuh)
+    bool unstable = false;                       // completion search: run 1 also finds every document's unstable tail
     const uint8_t *sp_flags = nullptr;           // host: per special 1 = allowed, 2 = disallowed (NULL: no special handling)
 };
 
@@ -858,6 +903,15 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
                                                                                       S.w_kdrop.p, S.w_btail.p, S.d_bytes, S.d_ctr);
             launches++;
         }
+        if (a.unstable && n_docs) {  // the tokens and offsets are final: L, |U| and the search items of every document
+            CUDA_TRY(S.w_kdrop.ensure((size_t)n_docs + 2)); CUDA_TRY(S.w_ulen.ensure((size_t)n_docs + 2));
+            CUDA_TRY(S.w_unit.ensure((size_t)n_docs + 2));
+            unstable_walk_kernel<<<(unsigned)((n_docs * 32 + 255) / 256), 256, 0, st>>>(a.d_doc_off, n_docs, S.w_pbits.p, sbits, a.d_out,
+                                                                                       a.d_tok_off, D->d_tok_boff, D->ut.space, h->n_ids,
+                                                                                       D->ut.max_len, S.w_kdrop.p, S.w_ulen.p,
+                                                                                       S.w_unit.p, S.d_ctr);
+            launches++;
+        }
         finalize_kernel<<<1, 32, 0, st>>>(S.d_ctr, S.d_sticky, a.d_counts, n_docs);
         launches += (sparse_docs ? 12 : 11) + (memo_slots ? 1 : 0);
     }
@@ -1032,6 +1086,23 @@ static void enqueue_scan(const uint32_t *cnt, uint64_t n, unsigned long long *pa
     scan_final_kernel<<<(unsigned)nb, 256, 0, st>>>(cnt, (long long)n, part, base, ctr);
 }
 
+// A second run of the pipeline over text built on the device (bytes mode, completion search): enqueue, wait, and grow
+// and re-run while a work-space was too small; the long-piece classes and miss memo counters of the run are added.
+static int run_again(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a, uint64_t *cls, uint64_t *memo, uint32_t *grown,
+                     uint32_t *reruns) {
+    int rc = enqueue_pipeline(h, D, S, a);
+    if (!rc) rc = collect_pipeline(h, S, nullptr, nullptr, grown);
+    for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {   // a work-space grew: the same run again
+        rc = enqueue_pipeline(h, D, S, a);
+        if (!rc) { (*reruns)++; rc = collect_pipeline(h, S, nullptr, nullptr, grown); }
+    }
+    if (rc == B200BPE_RETRY) rc = fail(B200BPE_ECUDA, "work-space sizing did not converge");
+    if (rc) return rc;
+    for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
+    add_miss_memo(S, memo);
+    return B200BPE_OK;
+}
+
 // Bytes mode, a chunk whose run 1 (a1, counters in S.h_ctr and S.h_bytes) found documents that are not well-formed UTF-8: run 2 encodes
 // the unstable piece [u_d, end_d) of every such document as one piece, then the splice puts each document's run-1 tokens
 // minus the last kdrop[d] in front of its run-2 tokens.  The final tokens and offsets end up in S.w_out / S.w_tokoff and
@@ -1055,17 +1126,9 @@ static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, u
     PipeArgs a2;
     a2.d_text = S.w_btext.p; a2.n_bytes = tail; a2.d_doc_off = S.w_b2doc.p; a2.n_docs = nd;
     a2.d_out = S.w_b2out.p; a2.d_tok_off = S.w_b2off.p; a2.st = st; a2.single_piece = true;
-    int rc = enqueue_pipeline(h, D, S, a2);
-    if (!rc) rc = collect_pipeline(h, S, nullptr, nullptr, grown);
-    for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {   // a work-space grew: run 2 again
-        rc = enqueue_pipeline(h, D, S, a2);
-        if (!rc) { (*reruns)++; rc = collect_pipeline(h, S, nullptr, nullptr, grown); }
-    }
-    if (rc == B200BPE_RETRY) rc = fail(B200BPE_ECUDA, "work-space sizing did not converge");
+    int rc = run_again(h, D, S, a2, cls, memo, grown, reruns);
     if (rc) return rc;
     float ms2 = 0; cudaEventElapsedTime(&ms2, S.ev[15], S.ev[4]);
-    for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
-    add_miss_memo(S, memo);
     const uint32_t launches2 = S.last_launches;
     *nt = n1 - drop + S.h_ctr->total_tokens;
     CUDA_TRY(S.w_bout.ensure((size_t)std::max<uint64_t>(*nt, a1.n_bytes) + 64));
@@ -1082,13 +1145,311 @@ static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, u
     return B200BPE_OK;
 }
 
+// ---- completion search (b200bpe_encode_with_unstable_batch, kernels_unstable.cuh) ------------------------------------
+
+// byte_pair_encode (src/lib.rs:198-210) of one byte string on the host, through the engine's own pair table: the literal
+// loop of _byte_pair_merge (smallest rank, leftmost on ties).  A byte the vocabulary lacks stays a PSEUDO_BASE id.
+static void host_byte_pair_encode(const DevTables &T, const std::string &b, std::vector<uint32_t> &ids) {
+    const size_t n = b.size();
+    ids.resize(n);
+    for (size_t j = 0; j < n; j++) ids[j] = T.byte_id[(uint8_t)b[j]];
+    std::vector<uint32_t> rk(n);
+    auto rank_at = [&](size_t j) { return j + 1 < ids.size() ? pair_lookup(T, ids[j], ids[j + 1]) : RANK_MAX; };
+    for (size_t j = 0; j < n; j++) rk[j] = rank_at(j);
+    for (;;) {
+        uint32_t best = RANK_MAX; size_t bj = 0;
+        for (size_t j = 0; j < ids.size(); j++) if (rk[j] < best) { best = rk[j]; bj = j; }
+        if (best == RANK_MAX) break;
+        ids[bj] = best;                           // the merged token's id is its rank
+        ids.erase(ids.begin() + (long)bj + 1); rk.erase(rk.begin() + (long)bj + 1);
+        rk[bj] = rank_at(bj);
+        if (bj) rk[bj - 1] = rank_at(bj - 1);
+    }
+}
+
+// The host side of the completion search tables (once per engine, under h->mu).
+static void unstable_host_build(b200bpe *h) {
+    auto &u = h->uh;
+    if (u.built) return;
+    const HostTables &H = h->H;
+    const DevTables T = H.view();
+    u.sorted.clear();
+    for (auto &kv : H.decoder) u.sorted.push_back(kv.first);
+    std::sort(u.sorted.begin(), u.sorted.end(), [&](uint32_t a, uint32_t b) { return H.decoder.at(a) < H.decoder.at(b); });
+    u.lenpre.assign(u.sorted.size() + 1, 0);
+    for (size_t i = 0; i < u.sorted.size(); i++) u.lenpre[i + 1] = u.lenpre[i] + H.decoder.at(u.sorted[i]).size();
+    u.space.assign((size_t)h->n_ids / 32 + 2, 0);
+    u.u8info.assign((size_t)h->n_ids + 1, 0);
+    u.ur_idx.assign((size_t)h->n_ids + 1, UR_NONE);
+    u.ur_off.assign(1, 0); u.ur_tok.clear();
+    u.max_len = 0;
+    std::vector<uint32_t> ids, zero;
+    for (uint32_t id : u.sorted) {
+        const std::string &b = H.decoder.at(id);
+        u.max_len = std::max<uint32_t>(u.max_len, (uint32_t)b.size());
+        bool all = !b.empty();
+        for (char c : b) all &= c == ' ' || c == '\n' || c == '\t';
+        if (all) u.space[id >> 5] |= 1u << (id & 31);
+        uint32_t c = 0;                           // leading continuation bytes; is the rest well-formed on its own?
+        while (c < b.size() && c < 4 && ((uint8_t)b[c] & 0xC0u) == 0x80u) c++;
+        bool rest_ok = true;
+        if (c < 4) {
+            const uint8_t *r = (const uint8_t *)b.data() + c;
+            const int64_t rn = (int64_t)b.size() - c;
+            zero.assign((size_t)(rn / 32) + 3, 0);
+            zero[0] = 1u;                         // one document that starts at byte 0
+            for (int64_t w = 0; w * 32 < rn && rest_ok; w++) rest_ok = utf8_bad_word(r, rn, zero.data(), w) == 0;
+        }
+        u.u8info[id] = (uint8_t)(c | (rest_ok ? 8u : 0u));
+        if (b.size() >= 2) {
+            host_byte_pair_encode(T, b, ids);
+            if (!(ids.size() == 1 && ids[0] == id)) {   // a token its own merges do not reach
+                u.ur_idx[id] = (uint32_t)(u.ur_off.size() - 1);
+                u.ur_tok.insert(u.ur_tok.end(), ids.begin(), ids.end());
+                u.ur_off.push_back((uint32_t)u.ur_tok.size());
+            }
+        }
+    }
+    u.built = true;
+}
+
+// The device side: one arena per device (under h->mu).
+static int unstable_upload(b200bpe *h, DevCtx *D) {
+    if (D->d_ut_arena) return B200BPE_OK;
+    const auto &u = h->uh;
+    struct Part { const void *src; size_t bytes; size_t off; };
+    std::vector<uint32_t> one(1, 0);
+    Part parts[] = {{u.sorted.data(), u.sorted.size() * 4, 0}, {u.lenpre.data(), u.lenpre.size() * 8, 0},
+                    {u.space.data(), u.space.size() * 4, 0}, {u.u8info.data(), u.u8info.size(), 0},
+                    {u.ur_idx.data(), u.ur_idx.size() * 4, 0}, {u.ur_off.data(), u.ur_off.size() * 4, 0},
+                    {u.ur_tok.empty() ? one.data() : u.ur_tok.data(), std::max<size_t>(u.ur_tok.size(), 1) * 4, 0}};
+    size_t total = 0;
+    for (auto &p : parts) { p.off = total; total += (p.bytes + 255) & ~(size_t)255; }
+    CUDA_TRY(cudaSetDevice(D->device));
+    UnstWs &W = D->uw;
+    if (!W.d_uc) CUDA_TRY(cudaMalloc((void **)&W.d_uc, sizeof(UnstCounters)));
+    if (!W.h_uc) CUDA_TRY(cudaHostAlloc((void **)&W.h_uc, sizeof(UnstCounters), cudaHostAllocPortable));
+    if (!W.d_sctr) CUDA_TRY(cudaMalloc((void **)&W.d_sctr, sizeof(Counters)));
+    uint8_t *arena = nullptr;
+    CUDA_TRY(cudaMalloc((void **)&arena, total));
+    for (auto &p : parts)
+        if (p.bytes) {
+            cudaError_t e = cudaMemcpy(arena + p.off, p.src, p.bytes, cudaMemcpyHostToDevice);
+            if (e != cudaSuccess) { cudaFree(arena); return fail(B200BPE_ECUDA, std::string("completion tables: ") + cudaGetErrorString(e)); }
+        }
+    D->d_ut_arena = arena;
+    UnstTables &U = D->ut;
+    U.sorted = (const uint32_t *)(arena + parts[0].off); U.n_sorted = (uint32_t)u.sorted.size();
+    U.lenpre = (const unsigned long long *)(arena + parts[1].off);
+    U.space = (const uint32_t *)(arena + parts[2].off);
+    U.u8info = arena + parts[3].off;
+    U.ur_idx = (const uint32_t *)(arena + parts[4].off);
+    U.ur_off = (const uint32_t *)(arena + parts[5].off);
+    U.ur_tok = (const uint32_t *)(arena + parts[6].off);
+    U.tok_boff = D->d_tok_boff; U.tok_blob = D->d_tok_blob; U.n_ids = h->n_ids; U.max_len = u.max_len;
+    return B200BPE_OK;
+}
+
+// grow a buffer that holds `used` elements to at least n, keeping them
+template <class Tp>
+static cudaError_t grow_keep(DevBuf<Tp> &b, size_t used, size_t n, cudaStream_t st) {
+    if (n <= b.cap) return cudaSuccess;
+    DevBuf<Tp> nb;
+    cudaError_t e = nb.ensure(std::max(n, 2 * b.cap));
+    if (e == cudaSuccess && used) e = cudaMemcpyAsync(nb.p, b.p, used * sizeof(Tp), cudaMemcpyDeviceToDevice, st);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+    if (e != cudaSuccess) { nb.release(); return e; }
+    b.release();
+    b = nb;
+    return cudaSuccess;
+}
+
+// exclusive scan of n u32 counts into base[0..n] (base[n] = the sum)
+static void uscan(UnstWs &W, const uint32_t *cnt, uint64_t n, unsigned long long *base, cudaStream_t st) {
+    if (n == 0) { cudaMemsetAsync(base, 0, 8, st); return; }
+    enqueue_scan(cnt, n, W.part.p, base, W.d_sctr, st);
+}
+
+struct UChunk {                  // one chunk's completions on the host
+    std::vector<uint32_t> tok; std::vector<uint64_t> off, grp;   // off: n_comp + 1, grp: n_docs + 1
+};
+
+// Completion search of one chunk whose run 1 (a1, with the walk) has been collected: splices the stable tokens (run 1
+// minus each document's last L) into S.w_out / S.w_tokoff (*nt = their count), then searches, encodes, truncates and
+// deduplicates the candidates in rounds and brings the chunk's completions home.  stats: documents with unstable bytes,
+// candidates encoded, candidates through byte_pair_encode, rounds, completions.
+static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, UChunk &out, uint64_t *stats, uint64_t *nt,
+                           uint64_t *cls, uint64_t *memo, uint32_t *grown, uint32_t *reruns) {
+    UnstWs &W = D->uw;
+    const UnstTables &U = D->ut;
+    const uint64_t nd = a1.n_docs;
+    cudaStream_t st = a1.st;
+    const float ms1[9] = {S.last_ms[0], S.last_ms[1], S.last_ms[2], S.last_ms[3], S.last_ms[4], S.last_ms[5], S.last_ms[6],
+                          S.last_ms[7], S.last_ms[8]};
+    const uint32_t launches1 = S.last_launches;
+    out.tok.clear(); out.off.assign(1, 0); out.grp.assign((size_t)nd + 1, 0);
+    if (nd == 0) return B200BPE_OK;
+    const uint64_t n1 = *nt;
+    // ---- stable tokens: run 1 minus the last L of every document (the bytes mode's splice with an empty run 2)
+    CUDA_TRY(S.w_btail.ensure((size_t)nd + 2)); CUDA_TRY(S.w_bbase.ensure((size_t)nd + 2));
+    CUDA_TRY(S.w_bpart.ensure((size_t)(nd / SCAN_ITEMS) + 4));
+    CUDA_TRY(S.w_bout.ensure((size_t)std::max<uint64_t>(n1, a1.n_bytes) + 64));
+    CUDA_TRY(W.zeros.ensure((size_t)nd + 2));
+    if (!S.d_bctr) CUDA_TRY(cudaMalloc((void **)&S.d_bctr, sizeof(Counters)));
+    CUDA_TRY(cudaMemsetAsync(W.zeros.p, 0, ((size_t)nd + 2) * 8, st));
+    bytes_count_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, st>>>(S.w_tokoff.p, W.zeros.p, S.w_kdrop.p, nd, S.w_btail.p);
+    enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_bbase.p, S.d_bctr, st);
+    bytes_splice_kernel<<<(unsigned)std::min<uint64_t>(nd, (uint64_t)D->n_sm * 16), 256, 0, st>>>(
+        S.w_out.p, S.w_tokoff.p, S.w_out.p, W.zeros.p, S.w_kdrop.p, S.w_bbase.p, nd, S.w_bout.p);
+    std::swap(S.w_out, S.w_bout);
+    std::swap(S.w_tokoff, S.w_bbase);
+    // ---- search items: (a), the (b) suffixes, (c) per document with unstable bytes
+    CUDA_TRY(W.item_base.ensure((size_t)nd + 2));
+    CUDA_TRY(W.part.ensure((size_t)(nd / SCAN_ITEMS) + 4));
+    CUDA_TRY(cudaMemsetAsync(W.d_uc, 0, sizeof(UnstCounters), st));
+    uscan(W, S.w_unit.p, nd, W.item_base.p, st);
+    CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.item_base.p + nd, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[1], S.w_tokoff.p + nd, 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    *nt = W.h_uc->tot[1];
+    const uint64_t n_items = W.h_uc->tot[0];
+    uint64_t n_cand = 0;
+    if (n_items) {
+        CUDA_TRY(W.it_lo.ensure((size_t)n_items + 2)); CUDA_TRY(W.it_cnt.ensure((size_t)n_items + 2));
+        CUDA_TRY(W.it_bytes.ensure((size_t)n_items + 2)); CUDA_TRY(W.it_doc.ensure((size_t)n_items + 2));
+        CUDA_TRY(W.cbase.ensure((size_t)n_items + 2)); CUDA_TRY(W.tbase.ensure((size_t)n_items + 2));
+        CUDA_TRY(W.part.ensure((size_t)(n_items / SCAN_ITEMS) + 4));
+        unstable_search_kernel<<<(unsigned)((nd * 32 + 255) / 256), 256, 0, st>>>(U, a1.d_text, a1.d_doc_off, nd, S.w_ulen.p,
+                                                                                 W.item_base.p, W.it_lo.p, W.it_cnt.p, W.it_bytes.p,
+                                                                                 W.it_doc.p, W.d_uc);
+        uscan(W, W.it_cnt.p, n_items, W.cbase.p, st);
+        uscan(W, W.it_bytes.p, n_items, W.tbase.p, st);
+        CUDA_TRY(cudaMemcpyAsync(W.h_uc, W.d_uc, sizeof(UnstCounters), cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.cbase.p + n_items, 8, cudaMemcpyDeviceToHost, st));
+        CUDA_TRY(cudaStreamSynchronize(st));
+        if (W.h_uc->err & UERR_BIG) return fail(B200BPE_EINVAL, "the completion candidates of one document need 4 GiB of text or more");
+        n_cand = W.h_uc->tot[0];
+        stats[0] += W.h_uc->n_docs;
+    }
+    if (n_cand >= 0xFFFFFFF0ull) return fail(B200BPE_EINVAL, "too many completion candidates in one chunk (2^32)");
+    UnstItems I;
+    I.doc_off = a1.d_doc_off; I.ulen = S.w_ulen.p; I.item_base = W.item_base.p; I.lo = W.it_lo.p; I.cnt = W.it_cnt.p;
+    I.doc = W.it_doc.p; I.cbase = W.cbase.p; I.tbase = W.tbase.p; I.n_items = n_items;
+    // rounds: at most one chunk of candidate text (B200BPE_CHUNK_MB) and a 32nd of that in candidates
+    const uint64_t cap = h->chunk_bytes, max_n = std::max<uint64_t>(cap / 32, 4096);
+    CUDA_TRY(W.grp.ensure((size_t)nd + 2)); CUDA_TRY(W.grp_off.ensure((size_t)nd + 2));
+    uint64_t n_comp = 0, n_tok = 0, rounds = 0, enc = 0, bpe = 0;
+    for (int attempt = 0;; attempt++) {
+        uint32_t slots = 4096;
+        while (slots < std::min<uint64_t>(2 * n_cand, 1u << 24)) slots <<= 1;
+        slots = std::max(slots, W.tslots_min);
+        CUDA_TRY(W.tkey.ensure(slots)); CUDA_TRY(W.tidx.ensure(slots)); CUDA_TRY(W.tloc.ensure(slots));
+        CUDA_TRY(cudaMemsetAsync(W.tkey.p, 0, (size_t)slots * 8, st));
+        CUDA_TRY(cudaMemsetAsync(W.tidx.p, 0xFF, (size_t)slots * 4, st));
+        CUDA_TRY(cudaMemsetAsync(W.grp.p, 0, ((size_t)nd + 2) * 4, st));
+        UnstTable T{W.tkey.p, W.tidx.p, W.tloc.p, slots - 1};
+        const unsigned long long seed = 0x9E3779B97F4A7C15ull * (unsigned long long)(attempt + 1);
+        n_comp = n_tok = rounds = enc = bpe = 0;
+        uint32_t err = 0;
+        for (uint64_t c0 = 0; c0 < n_cand && !err;) {
+            CUDA_TRY(cudaMemsetAsync(W.d_uc, 0, sizeof(UnstCounters), st));
+            unstable_round_kernel<<<1, 32, 0, st>>>(U, I, n_cand, c0, max_n, cap, W.d_uc);
+            CUDA_TRY(cudaMemcpyAsync(&W.h_uc->round, &W.d_uc->round, sizeof(W.h_uc->round), cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            const uint64_t c1 = W.h_uc->round[0], nr = c1 - c0;
+            CUDA_TRY(W.cinfo.ensure((size_t)nr + 2)); CUDA_TRY(W.o_len.ensure((size_t)nr + 2)); CUDA_TRY(W.s_len.ensure(2 * (size_t)nr + 2));
+            CUDA_TRY(W.o_off.ensure((size_t)nr + 2)); CUDA_TRY(W.s_off.ensure(2 * (size_t)nr + 2));
+            CUDA_TRY(W.tokoff_o.ensure((size_t)nr + 2)); CUDA_TRY(W.tokoff_s.ensure(2 * (size_t)nr + 2));
+            CUDA_TRY(W.nkeep.ensure((size_t)nr + 2)); CUDA_TRY(W.slot.ensure((size_t)nr + 2)); CUDA_TRY(W.keep.ensure((size_t)nr + 2));
+            CUDA_TRY(W.kc.ensure((size_t)nr + 2)); CUDA_TRY(W.rcb.ensure((size_t)nr + 2)); CUDA_TRY(W.rtb.ensure((size_t)nr + 2));
+            CUDA_TRY(W.part.ensure((size_t)(2 * nr / SCAN_ITEMS) + 4));
+            const unsigned grid = (unsigned)((nr + 255) / 256);
+            unstable_meta_kernel<<<grid, 256, 0, st>>>(U, I, a1.d_text, c0, nr, W.cinfo.p, W.o_len.p, W.s_len.p, W.d_uc);
+            uscan(W, W.o_len.p, nr, W.o_off.p, st);
+            uscan(W, W.s_len.p, 2 * nr, W.s_off.p, st);
+            CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.o_off.p + nr, 8, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[1], W.s_off.p + 2 * nr, 8, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            const uint64_t ob = W.h_uc->tot[0], sb = W.h_uc->tot[1];
+            // run 2: encode_ordinary of the UTF-8 candidates, single-piece mode for the others and the parts of (c)
+            if (ob) {
+                CUDA_TRY(W.text_o.ensure((size_t)ob + 64)); CUDA_TRY(W.out_o.ensure((size_t)ob + 64));
+                unstable_gather_kernel<<<(unsigned)((ob + 16 * 256 - 1) / (16 * 256)), 256, 0, st>>>(
+                    U, a1.d_text, a1.d_doc_off, S.w_ulen.p, W.cinfo.p, nr, 1, W.o_off.p, W.text_o.p);
+                PipeArgs a2;
+                a2.d_text = W.text_o.p; a2.n_bytes = ob; a2.d_doc_off = W.o_off.p; a2.n_docs = nr;
+                a2.d_out = W.out_o.p; a2.d_tok_off = W.tokoff_o.p; a2.st = st;
+                int rc = run_again(h, D, S, a2, cls, memo, grown, reruns);
+                if (rc) return rc;
+            } else CUDA_TRY(cudaMemsetAsync(W.tokoff_o.p, 0, ((size_t)nr + 1) * 8, st));
+            if (sb) {
+                CUDA_TRY(W.text_s.ensure((size_t)sb + 64)); CUDA_TRY(W.out_s.ensure((size_t)sb + 64));
+                unstable_gather_kernel<<<(unsigned)((sb + 16 * 256 - 1) / (16 * 256)), 256, 0, st>>>(
+                    U, a1.d_text, a1.d_doc_off, S.w_ulen.p, W.cinfo.p, nr, 2, W.s_off.p, W.text_s.p);
+                PipeArgs a3;
+                a3.d_text = W.text_s.p; a3.n_bytes = sb; a3.d_doc_off = W.s_off.p; a3.n_docs = 2 * nr;
+                a3.d_out = W.out_s.p; a3.d_tok_off = W.tokoff_s.p; a3.st = st; a3.single_piece = true;
+                int rc = run_again(h, D, S, a3, cls, memo, grown, reruns);
+                if (rc) return rc;
+            } else CUDA_TRY(cudaMemsetAsync(W.tokoff_s.p, 0, (2 * (size_t)nr + 1) * 8, st));
+            // truncate, deduplicate, append
+            RunOut R{W.out_o.p, W.tokoff_o.p, W.out_s.p, W.tokoff_s.p};
+            UnstResult res{W.res_tok.p, W.res_off.p, W.res_doc.p, W.grp.p};
+            CUDA_TRY(cudaMemsetAsync(S.d_bctr, 0, sizeof(Counters), st));
+            unstable_insert_kernel<<<grid, 256, 0, st>>>(U, R, W.cinfo.p, S.w_ulen.p, c0, nr, seed, T, W.nkeep.p, W.slot.p, W.d_uc, S.d_bctr);
+            unstable_verify_kernel<<<grid, 256, 0, st>>>(U, R, W.cinfo.p, c0, nr, T, res, W.nkeep.p, W.slot.p, W.keep.p, W.kc.p, W.d_uc);
+            uscan(W, W.keep.p, nr, W.rcb.p, st);
+            uscan(W, W.kc.p, nr, W.rtb.p, st);
+            CUDA_TRY(cudaMemcpyAsync(W.h_uc, W.d_uc, sizeof(UnstCounters), cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.rcb.p + nr, 8, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[1], W.rtb.p + nr, 8, cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaMemcpyAsync(S.h_ctr, S.d_bctr, sizeof(Counters), cudaMemcpyDeviceToHost, st));
+            CUDA_TRY(cudaStreamSynchronize(st));
+            CUDA_TRY(cudaGetLastError());
+            if (S.h_ctr->err & ERR_NOBYTE)
+                return fail(B200BPE_ENOBYTE, "a piece needs a single-byte token that mergeable_ranks does not contain");
+            err = W.h_uc->err;
+            if (err) break;
+            enc += W.h_uc->n_encoded; bpe += W.h_uc->n_bpe;
+            const uint64_t kept = W.h_uc->tot[0], toks = W.h_uc->tot[1];
+            CUDA_TRY(grow_keep(W.res_tok, (size_t)n_tok, (size_t)(n_tok + toks) + 1, st));
+            CUDA_TRY(grow_keep(W.res_off, (size_t)(n_comp ? n_comp + 1 : 0), (size_t)(n_comp + kept) + 2, st));
+            CUDA_TRY(grow_keep(W.res_doc, (size_t)n_comp, (size_t)(n_comp + kept) + 1, st));
+            res = UnstResult{W.res_tok.p, W.res_off.p, W.res_doc.p, W.grp.p};
+            unstable_write_kernel<<<grid, 256, 0, st>>>(U, R, W.cinfo.p, nr, T, res, W.keep.p, W.kc.p, W.slot.p, W.rcb.p, W.rtb.p,
+                                                        n_comp, n_tok);
+            n_comp += kept; n_tok += toks; rounds++;
+            c0 = c1;
+        }
+        if (!err) break;
+        if (attempt >= 3) return fail(B200BPE_ECUDA, "completion deduplication did not converge");
+        if (err & UERR_TABLE) W.tslots_min = slots * 4;   // else UERR_COLLIDE: the next attempt has another seed
+        (*reruns)++;
+    }
+    // ---- the chunk's completions: tokens, completion boundaries, per-document ranges
+    CUDA_TRY(grow_keep(W.res_off, (size_t)(n_comp ? n_comp + 1 : 0), (size_t)n_comp + 2, st));
+    W.h_uc->tot[2] = n_tok;
+    CUDA_TRY(cudaMemcpyAsync(W.res_off.p + n_comp, &W.h_uc->tot[2], 8, cudaMemcpyHostToDevice, st));
+    uscan(W, W.grp.p, nd, W.grp_off.p, st);
+    out.tok.resize((size_t)n_tok); out.off.resize((size_t)n_comp + 1);
+    if (n_tok) CUDA_TRY(cudaMemcpyAsync(out.tok.data(), W.res_tok.p, (size_t)n_tok * 4, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out.off.data(), W.res_off.p, ((size_t)n_comp + 1) * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaMemcpyAsync(out.grp.data(), W.grp_off.p, ((size_t)nd + 1) * 8, cudaMemcpyDeviceToHost, st));
+    CUDA_TRY(cudaStreamSynchronize(st));
+    CUDA_TRY(cudaGetLastError());
+    stats[1] += enc; stats[2] += bpe; stats[3] += rounds; stats[4] += n_comp;
+    memcpy(S.last_ms, ms1, sizeof(ms1));
+    S.last_launches = launches1;
+    return B200BPE_OK;
+}
+
 // --------------------------------------------------------------------------------------------
 // host path: host buffers in, ONE pinned result out; chunks round-robin over the devices
 // --------------------------------------------------------------------------------------------
 struct HostJob {
     b200bpe *h = nullptr;
     const uint8_t *text = nullptr; const uint64_t *doc_off = nullptr; uint64_t n_docs = 0;
-    bool single_piece = false, pageable = false, bytes = false;
+    bool single_piece = false, pageable = false, bytes = false, unstable = false;
     const uint8_t *sp_flags = nullptr;
     std::vector<uint64_t> cut;                    // chunk c = documents [cut[c], cut[c+1])
     std::vector<std::atomic<long long>> count;    // tokens of chunk c, -1 until its kernels are done
@@ -1100,6 +1461,8 @@ struct HostJob {
     uint32_t grown = 0, reruns = 0;               // B200BPE_GREW_* bits / pipeline re-runs of all workers (under stat_mu)
     uint64_t cls[N_CLS] = {};                     // long pieces per length class of the chunks' final runs (under stat_mu)
     uint64_t bytes_repairs = 0;                   // bytes mode: documents repaired (under stat_mu)
+    std::vector<UChunk> uch;                      // completion search: chunk c's completions
+    uint64_t ustats[5] = {};                      // completion search: b200bpe_last_unstable (under stat_mu)
     uint64_t memo[3] = {};                        // miss memo counters of the chunks' final runs (under stat_mu)
 
     void set_error(int rc) {
@@ -1202,13 +1565,13 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         PipeArgs a;
         a.d_text = S.w_text.p; a.n_bytes = doc_off[hi] - doc_off[lo]; a.d_doc_off = S.w_docoff.p; a.n_docs = hi - lo;
         a.d_out = S.w_out.p; a.d_tok_off = S.w_tokoff.p; a.st = S.stream; a.single_piece = J->single_piece; a.sp_flags = J->sp_flags;
-        a.bytes = J->bytes;
+        a.bytes = J->bytes; a.unstable = J->unstable;
         return a;
     };
     size_t known = 0; uint64_t known_sum = 0;                    // prefix of the per-chunk token counts seen so far
     float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; float last_d2h = 0;
     uint32_t grown = 0, reruns = 0;
-    uint64_t cls[N_CLS] = {}, repaired = 0, memo[3] = {};
+    uint64_t cls[N_CLS] = {}, repaired = 0, memo[3] = {}, ustats[5] = {};
     // finalise chunk k: wait for its kernels, then send its offsets + tokens home (async) at their final place
     auto drain = [&](size_t k) -> int {
         Slot &S = slot_of(k);
@@ -1234,6 +1597,10 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         if (J->bytes && S.h_bytes->n_docs) {                     // documents that are not well-formed UTF-8: run 2 + splice
             repaired += S.h_bytes->n_docs;
             rc = bytes_tail_runs(h, D, S, args_of(k), &nt, cls, memo, &grown, &reruns);
+            if (rc) return rc;
+        }
+        if (J->unstable) {                                       // stable tokens + the chunk's completions
+            rc = unstable_search(h, D, S, args_of(k), J->uch[c], ustats, &nt, cls, memo, &grown, &reruns);
             if (rc) return rc;
         }
         J->count[c].store((long long)nt);
@@ -1281,13 +1648,16 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     const size_t AHEAD = (size_t)DevCtx::N_SLOTS - 2;
     int rc = B200BPE_OK;
     for (size_t k = 0; k < AHEAD && k < mine.size(); k++) { rc = enqueue_h2d(k); if (rc) return bail(rc); }
+    // The completion search of a chunk waits for the device several times per round, so it does not run next to the next
+    // chunk's kernels: each chunk is drained before the next one starts (uploads still run ahead).
+    const size_t lag = J->unstable ? 0 : 1;
     for (size_t k = 0; k < mine.size() && !stop(); k++) {
         if (k + AHEAD < mine.size()) { rc = enqueue_h2d(k + AHEAD); if (rc) return bail(rc); }
         rc = enqueue_pipeline(h, D, slot_of(k), args_of(k));
         if (rc) return bail(rc);
-        if (k >= 1) { rc = drain(k - 1); if (rc) return bail(rc); }   // overlaps with chunk k's kernels
+        if (k >= lag) { rc = drain(k - lag); if (rc) return bail(rc); }   // overlaps with chunk k's kernels (lag 1)
     }
-    if (!stop()) { rc = drain(mine.size() - 1); if (rc) return bail(rc); }
+    if (lag && !stop()) { rc = drain(mine.size() - 1); if (rc) return bail(rc); }
     bail(0);
     if (!stop()) { Slot &S = slot_of(mine.size() - 1); cudaEventElapsedTime(&last_d2h, S.ev[5], S.ev[6]); }
     std::lock_guard<std::mutex> lk(J->stat_mu);
@@ -1297,11 +1667,13 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     J->grown |= grown; J->reruns += reruns;
     for (int i = 0; i < N_CLS; i++) J->cls[i] += cls[i];
     J->bytes_repairs += repaired;
+    for (int i = 0; i < 5; i++) J->ustats[i] += ustats[i];
     for (int i = 0; i < 3; i++) J->memo[i] += memo[i];
 }
 
 static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, bool single_piece,
-                       const uint8_t *sp_flags, b200bpe_result **out, int *special_idx, bool bytes = false) {
+                       const uint8_t *sp_flags, b200bpe_result **out, int *special_idx, bool bytes = false,
+                       b200bpe_result **completions = nullptr) {
     const uint64_t n_bytes = doc_off[n_docs];
     if (doc_off[0] != 0) return fail(B200BPE_EINVAL, "document offsets must start at 0");
     const int n_dev = (int)h->devs.size();
@@ -1339,7 +1711,8 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
     for (int pass = 0; pass < 2; pass++) {
         HostJob J;
         J.h = h; J.text = text; J.doc_off = doc_off; J.n_docs = n_docs; J.single_piece = single_piece; J.pageable = pageable;
-        J.sp_flags = sp_flags; J.cut = cut; J.bytes = bytes;
+        J.sp_flags = sp_flags; J.cut = cut; J.bytes = bytes; J.unstable = completions != nullptr;
+        if (J.unstable) J.uch.resize(n_chunks);
         J.count = std::vector<std::atomic<long long>>(n_chunks);
         for (auto &c : J.count) c.store(-1);
         b200bpe_result *r = new b200bpe_result();
@@ -1371,6 +1744,25 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
         h->set_piece_classes(J.cls);
         h->last_bytes_repairs = J.bytes_repairs;
         h->set_miss_memo(J.memo);
+        if (completions) {                                        // the chunks' completions, back to back
+            b200bpe_result *r2 = new b200bpe_result();
+            r2->owner = h; r2->on_host_vec = true;
+            size_t nt = 0, nc = 0;
+            for (auto &u : J.uch) { nt += u.tok.size(); nc += u.off.size() - 1; }
+            r2->vtok.reserve(nt); r2->voff.reserve(nc + 1); r2->vgrp.reserve((size_t)n_docs + 1);
+            r2->vgrp.push_back(0);
+            for (auto &u : J.uch) {
+                const uint64_t tb = r2->vtok.size(), cb = r2->voff.size();
+                r2->vtok.insert(r2->vtok.end(), u.tok.begin(), u.tok.end());
+                for (size_t q = 0; q + 1 < u.off.size(); q++) r2->voff.push_back(tb + u.off[q]);
+                for (size_t d = 1; d < u.grp.size(); d++) r2->vgrp.push_back(cb + u.grp[d]);
+            }
+            r2->voff.push_back(r2->vtok.size());
+            r2->n_tokens = r2->vtok.size(); r2->n_docs = r2->voff.size() - 1;
+            for (int i = 0; i < 5; i++) h->last_unstable[i] = J.ustats[i];
+            h->live_results++;
+            *completions = r2;
+        }
         h->live_results++;                                        // caller holds h->mu
         *out = r;
         return B200BPE_OK;
@@ -1440,6 +1832,30 @@ extern "C" int b200bpe_encode_batch(b200bpe_t *h, const uint8_t *text, const uin
     return b200bpe_encode_batch_special(h, text, doc_off, n_docs, allowed ? flags.data() : nullptr, out, nullptr);
 }
 
+// Encoding.encode_with_unstable (tiktoken/core.py:208-243 -> src/py.rs:117-131 -> CoreBPE::_encode_unstable_native,
+// src/lib.rs:483-599) for every document of a batch, the disallowed check included; kernels_unstable.cuh.
+extern "C" int b200bpe_encode_with_unstable_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
+                                                  const uint8_t *flags, b200bpe_result_t **stable,
+                                                  b200bpe_result_t **completions, int32_t *special_index) {
+    if (h) h->reset_reruns();
+    if (!h || !doc_off || !stable || !completions) return fail(B200BPE_EINVAL, "null argument");
+    if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
+    if (!h->decode_on_device)
+        return fail(B200BPE_EINVAL, "the completion search reads token bytes from the device decode tables: every token id must be < 2^24");
+    bool any = false;
+    if (flags) for (size_t i = 0; i < h->specials.size(); i++) any |= flags[i] != 0;
+    std::lock_guard<std::mutex> lk(h->mu);
+    DeviceGuard guard;
+    unstable_host_build(h);
+    for (auto *D : h->devs) { int rc = unstable_upload(h, D); if (rc) return rc; }
+    int sidx = -1;
+    b200bpe_result *comp = nullptr;
+    int rc = encode_host(h, text, doc_off, n_docs, false, any ? flags : nullptr, stable, &sidx, false, &comp);
+    if (rc == B200BPE_ESPECIAL && special_index) *special_index = sidx;
+    if (!rc) *completions = comp;
+    return rc;
+}
+
 extern "C" const char *b200bpe_special_name(b200bpe_t *h, int32_t index) {
     if (!h || index < 0 || (size_t)index >= h->specials.size()) return nullptr;
     return h->specials[(size_t)index].c_str();
@@ -1450,6 +1866,10 @@ extern "C" const uint32_t *b200bpe_result_tokens(const b200bpe_result_t *r) {
 }
 extern "C" const uint64_t *b200bpe_result_offsets(const b200bpe_result_t *r) {
     return r->on_host_vec ? r->voff.data() : (const uint64_t *)r->off.p;
+}
+extern "C" const uint64_t *b200bpe_result_groups(const b200bpe_result_t *r, uint64_t *n_groups) {
+    if (n_groups) *n_groups = r->vgrp.empty() ? 0 : r->vgrp.size() - 1;
+    return r->vgrp.empty() ? nullptr : r->vgrp.data();
 }
 extern "C" uint64_t b200bpe_result_n_tokens(const b200bpe_result_t *r) { return r->n_tokens; }
 extern "C" uint64_t b200bpe_result_n_docs(const b200bpe_result_t *r) { return r->n_docs; }
@@ -1626,6 +2046,12 @@ extern "C" int b200bpe_last_miss_memo(b200bpe_t *h, uint64_t *misses, uint64_t *
 extern "C" int b200bpe_last_bytes_repairs(b200bpe_t *h, uint64_t *n_docs_repaired) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
     if (n_docs_repaired) *n_docs_repaired = h->last_bytes_repairs.load();
+    return B200BPE_OK;
+}
+
+extern "C" int b200bpe_last_unstable(b200bpe_t *h, uint64_t *stats5) {
+    if (!h || !stats5) return fail(B200BPE_EINVAL, "null argument");
+    for (int i = 0; i < 5; i++) stats5[i] = h->last_unstable[i].load();
     return B200BPE_OK;
 }
 

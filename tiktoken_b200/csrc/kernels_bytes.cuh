@@ -100,6 +100,72 @@ __device__ __forceinline__ bool tok_all_space(const uint32_t *__restrict__ space
     return t < n_ids && ((__ldg(space_bits + (t >> 5)) >> (t & 31)) & 1u);
 }
 
+// The highest piece start in [start, v), 32 pbits words per warp step; start when there is none.  Every lane returns it.
+__device__ __forceinline__ unsigned long long last_piece_start(int lane, unsigned long long start, unsigned long long v,
+                                                               const uint32_t *__restrict__ pbits) {
+    long long p = -1;
+    for (long long wb = (long long)((v - 1) >> 5); wb >= (long long)(start >> 5) && p < 0; wb -= 32) {
+        const long long wi = wb - lane;
+        uint32_t m = 0;
+        if (wi >= (long long)(start >> 5)) {
+            m = pbits[wi];
+            const long long lo = (long long)start - wi * 32, hi = (long long)v - wi * 32;   // keep bits [lo, hi)
+            if (hi < 32) m &= (1u << hi) - 1u;
+            if (lo > 0) m &= ~((1u << lo) - 1u);
+        }
+        const uint32_t hit = __ballot_sync(0xFFFFFFFFu, m != 0);
+        if (hit) {
+            const int src = __ffs(hit) - 1;                  // the lane with the highest word
+            const uint32_t mw = __shfl_sync(0xFFFFFFFFu, m, src);
+            p = (wb - src) * 32 + (31 - __clz(mw));
+        }
+    }
+    return p < 0 ? start : (unsigned long long)p;
+}
+
+// The tokens [t0, t1) of a haystack end at byte v and its last piece starts at p: L = the tokens from t1 - 1 backwards
+// that cover [p, v), extended backwards over all-space tokens when the first of them is all-space
+// (_increase_last_piece_token_len, lib.rs:455-476); bytes = what the L tokens cover.  False when p is not a token
+// boundary (a kernel invariant).  One warp; every lane returns the same.
+__device__ __forceinline__ bool last_piece_tokens(int lane, unsigned long long p, unsigned long long v,
+                                                  const uint32_t *__restrict__ tokens, unsigned long long t0, unsigned long long t1,
+                                                  const uint32_t *__restrict__ tok_boff, const uint32_t *__restrict__ space_bits,
+                                                  uint32_t n_ids, unsigned long long &L_out, unsigned long long &bytes_out) {
+    const unsigned long long plen = v - p;
+    unsigned long long acc = 0, L = 0;
+    bool ok = true;
+    for (unsigned long long it = 0;; it += 32) {
+        const long long ti = (long long)t1 - 1 - (long long)it - lane;
+        const bool have = ti >= (long long)t0;
+        const uint32_t len = have ? tok_len(tok_boff, n_ids, tokens[ti]) : 0u;
+        const uint32_t inc = warp_incl_scan_u32(len, lane);
+        const uint32_t reach = __ballot_sync(0xFFFFFFFFu, have && acc + inc >= plen);
+        if (reach) {
+            const int j = __ffs(reach) - 1;
+            ok = acc + __shfl_sync(0xFFFFFFFFu, inc, j) == plen;   // a piece start is a token boundary
+            L = it + j + 1;
+            break;
+        }
+        if (!__all_sync(0xFFFFFFFFu, have)) { ok = false; break; }
+        acc += __shfl_sync(0xFFFFFFFFu, inc, 31);
+    }
+    unsigned long long bytes = plen;
+    if (ok && tok_all_space(space_bits, n_ids, tokens[t1 - L])) {   // _increase_last_piece_token_len
+        for (;;) {
+            const long long ti = (long long)(t1 - L) - 1 - lane;
+            const bool sp = ti >= (long long)t0 && tok_all_space(space_bits, n_ids, tokens[ti]);
+            const uint32_t len = sp ? tok_len(tok_boff, n_ids, tokens[ti]) : 0u;
+            const uint32_t run = ~__ballot_sync(0xFFFFFFFFu, sp);
+            const int n_sp = run ? __ffs(run) - 1 : 32;      // leading all-space tokens of this step
+            bytes += __reduce_add_sync(0xFFFFFFFFu, lane < n_sp ? len : 0u);
+            L += (unsigned long long)n_sp;
+            if (n_sp < 32) break;
+        }
+    }
+    L_out = L; bytes_out = bytes;
+    return ok;
+}
+
 // One warp per document, after run 1's gather.  For a damaged document: p = the last piece start in [start, v),
 // L = the tokens that cover [p, v), extended backwards over all-space tokens when the first of them is all-space
 // (lib.rs:455-476); k = L + 1 tokens to drop (the placeholder is the last), u = v - (bytes of the L tokens).
@@ -121,56 +187,9 @@ __global__ void __launch_bounds__(256) bytes_repair_kernel(const unsigned long l
     unsigned long long u = v, k = 1;
     bool ok = true;
     if (v > start) {
-        // p: highest piece start in [start, v), 32 words per step
-        long long p = -1;
-        for (long long wb = (long long)((v - 1) >> 5); wb >= (long long)(start >> 5) && p < 0; wb -= 32) {
-            const long long wi = wb - lane;
-            uint32_t m = 0;
-            if (wi >= (long long)(start >> 5)) {
-                m = pbits[wi];
-                const long long lo = (long long)start - wi * 32, hi = (long long)v - wi * 32;   // keep bits [lo, hi)
-                if (hi < 32) m &= (1u << hi) - 1u;
-                if (lo > 0) m &= ~((1u << lo) - 1u);
-            }
-            const uint32_t hit = __ballot_sync(0xFFFFFFFFu, m != 0);
-            if (hit) {
-                const int src = __ffs(hit) - 1;                  // the lane with the highest word
-                const uint32_t mw = __shfl_sync(0xFFFFFFFFu, m, src);
-                p = (wb - src) * 32 + (31 - __clz(mw));
-            }
-        }
-        if (p < 0) p = (long long)start;
-        // L: tokens from t1 - 1 backwards whose lengths add up to v - p
-        const unsigned long long plen = v - (unsigned long long)p;
-        unsigned long long acc = 0, L = 0;
-        for (unsigned long long it = 0;; it += 32) {
-            const long long ti = (long long)t1 - 1 - (long long)it - lane;
-            const bool have = ti >= (long long)t0;
-            const uint32_t len = have ? tok_len(tok_boff, n_ids, tokens[ti]) : 0u;
-            const uint32_t inc = warp_incl_scan_u32(len, lane);
-            const uint32_t reach = __ballot_sync(0xFFFFFFFFu, have && acc + inc >= plen);
-            if (reach) {
-                const int j = __ffs(reach) - 1;
-                ok = acc + __shfl_sync(0xFFFFFFFFu, inc, j) == plen;   // a piece start is a token boundary
-                L = it + j + 1;
-                break;
-            }
-            if (!__all_sync(0xFFFFFFFFu, have)) { ok = false; break; }
-            acc += __shfl_sync(0xFFFFFFFFu, inc, 31);
-        }
-        unsigned long long bytes = plen;
-        if (ok && tok_all_space(space_bits, n_ids, tokens[t1 - L])) {   // _increase_last_piece_token_len
-            for (;;) {
-                const long long ti = (long long)(t1 - L) - 1 - lane;
-                const bool sp = ti >= (long long)t0 && tok_all_space(space_bits, n_ids, tokens[ti]);
-                const uint32_t len = sp ? tok_len(tok_boff, n_ids, tokens[ti]) : 0u;
-                const uint32_t run = ~__ballot_sync(0xFFFFFFFFu, sp);
-                const int n_sp = run ? __ffs(run) - 1 : 32;      // leading all-space tokens of this step
-                bytes += __reduce_add_sync(0xFFFFFFFFu, lane < n_sp ? len : 0u);
-                L += (unsigned long long)n_sp;
-                if (n_sp < 32) break;
-            }
-        }
+        const unsigned long long p = last_piece_start(lane, start, v, pbits);
+        unsigned long long L = 0, bytes = 0;
+        ok = last_piece_tokens(lane, p, v, tokens, t0, t1, tok_boff, space_bits, n_ids, L, bytes);
         u = v - bytes;
         k = L + 1;
     }
