@@ -31,7 +31,10 @@ extern "C" {
 #define B200BPE_ESPECIAL -7   /* the text contains a disallowed special token (-> ValueError,
                                  tiktoken/core.py:120-124, :431-438)                           */
 #define B200BPE_ECAPACITY -8  /* a device work-space had to grow while several asynchronous device
-                                 calls were queued: re-issue them (b200bpe_device_wait)         */
+                                 calls were queued: re-issue them (b200bpe_device_wait); training: more
+                                 merges than the caller's merge buffer holds                      */
+#define B200BPE_ENOPAIR  -9   /* training: no pair is left to merge before vocab_size is reached (-> ValueError;
+                                 the reference's max() of an empty Counter, tiktoken/_educational.py:144) */
 
 typedef struct b200bpe b200bpe_t;
 typedef struct b200bpe_result b200bpe_result_t;
@@ -123,6 +126,23 @@ int b200bpe_encode_bytes_batch(b200bpe_t *h, const uint8_t *text, const uint64_t
 int b200bpe_encode_with_unstable_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                        const uint8_t *flags, b200bpe_result_t **stable, b200bpe_result_t **completions,
                                        int32_t *special_index);
+
+/* tiktoken._educational.bpe_train (tiktoken/_educational.py:119-185) over a batch of documents; needs no engine.
+ * text = concatenated UTF-8 of all documents, document d = [doc_off[d], doc_off[d+1]) (HOST buffers).  The words are the
+ * pat_str pieces of document 0, then document 1, ... (no piece crosses a document boundary).  pat_str must be one of the
+ * three patterns b200bpe_create accepts.  Starting from the 256 single bytes, each merge takes the adjacent pair of
+ * highest count over all words (ties: the pair whose first occurrence comes first, by word, then position), applies it
+ * left to right without overlap in every word, and gives the merged bytes the id len(ranks) -- or, when those bytes
+ * already are a token, that token's id, and len(ranks) does not grow -- until len(ranks) == vocab_size.
+ * merges_out receives 3 uint32 per merge: left id, right id, merged id (ids 0..255 are the bytes; a new id is the number
+ * of tokens so far); *n_merges_out their count.  At most merges_cap merges, else B200BPE_ECAPACITY.  No pair left
+ * before vocab_size: B200BPE_ENOPAIR.  vocab_size < 256: B200BPE_EINVAL.  Runs on CUDA device `device`, the merge loop
+ * without a host synchronisation per merge (a CUDA graph of B200BPE_TRAIN_GRAPH_STEPS merges, default 128, per host
+ * check).  stats8 (may be NULL): [0] pieces, [1] distinct words, [2] merges, [3] graph batches, device ms of [4] the
+ * split, [5] the distinct-word stage, [6] the merge loop, [7] chunks (B200BPE_CHUNK_MB, default 64 MiB). */
+int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, const char *pat_str,
+                      uint32_t vocab_size, int device, uint32_t *merges_out, uint64_t merges_cap,
+                      uint64_t *n_merges_out, double *stats8);
 
 /* Name of special token `index` (as given to b200bpe_create), or NULL. */
 const char *b200bpe_special_name(b200bpe_t *h, int32_t index);

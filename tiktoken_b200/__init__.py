@@ -7,6 +7,8 @@
     tiktoken_b200.get_encoding("cl100k_base")   # the reference's registry + plugins, GPU-backed Encoding
     tiktoken_b200.install()                     # or: run the UNMODIFIED `tiktoken` package on the GPU engine
 
+    tiktoken_b200.bpe_train(text, 50_000, pat)  # tiktoken._educational.bpe_train on the GPU (train.py)
+
 `tiktoken_b200._tiktoken.CoreBPE` is the drop-in for the Rust extension (see INTEGRATION.md).  Everything the
 north star says stays -- tiktoken/core.py's host class, tiktoken/registry.py, tiktoken/load.py, the tiktoken_ext
 plugins -- is the reference's own code, imported, not re-typed.
@@ -16,6 +18,7 @@ from __future__ import annotations
 import threading
 
 from .core import Encoding  # noqa: F401
+from .train import bpe_train, bpe_train_batch, bpe_train_packed, last_train_stats  # noqa: F401
 
 __version__ = "0.2.0"
 

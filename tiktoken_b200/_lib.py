@@ -15,10 +15,10 @@ import subprocess
 _CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 _SO = os.path.join(_CSRC, "libb200bpe.so")
 _SOURCES = ["b200bpe.cu", "dev_common.cuh", "kernels_pretok.cuh", "kernels_long.cuh", "kernels_mid.cuh", "kernels_pmerge.cuh", "kernels_encode.cuh",
-            "kernels_special.cuh", "kernels_decode.cuh", "kernels_bytes.cuh", "kernels_unstable.cuh", "utf8_check.cuh", "bpe_device.cuh", "bpe_tables.h", "pretok_rules.cuh",
+            "kernels_special.cuh", "kernels_decode.cuh", "kernels_bytes.cuh", "kernels_unstable.cuh", "kernels_train.cuh", "utf8_check.cuh", "bpe_device.cuh", "bpe_tables.h", "pretok_rules.cuh",
             "pretok_fast.cuh", "text_access.cuh", "unicode_classes.inc"]
 
-OK, EINVAL, EPATTERN, EDUPRANK, ECUDA, ENOBYTE, EKEY, ESPECIAL, ECAPACITY = 0, -1, -2, -3, -4, -5, -6, -7, -8
+OK, EINVAL, EPATTERN, EDUPRANK, ECUDA, ENOBYTE, EKEY, ESPECIAL, ECAPACITY, ENOPAIR = 0, -1, -2, -3, -4, -5, -6, -7, -8, -9
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-shared", "-Xcompiler", "-fPIC"]
@@ -114,6 +114,8 @@ def lib() -> C.CDLL:
     L.b200bpe_table_bytes.argtypes = [vp, vp]
     L.b200bpe_device_count.restype = i32
     L.b200bpe_device_count.argtypes = []
+    L.b200bpe_bpe_train.restype = i32
+    L.b200bpe_bpe_train.argtypes = [vp, vp, u64, C.c_char_p, u32, i32, vp, u64, C.POINTER(u64), vp]
     L.b200bpe_last_error.restype = C.c_char_p
     L.b200bpe_version.restype = C.c_char_p
     _lib = L
@@ -128,7 +130,7 @@ EXPORTS = [
     "b200bpe_version", "b200bpe_device_count", "b200bpe_create_multi", "b200bpe_n_devices", "b200bpe_encode_batch_special",
     "b200bpe_special_name", "b200bpe_encode_device_async", "b200bpe_device_wait", "b200bpe_trim", "b200bpe_last_reruns",
     "b200bpe_last_piece_classes", "b200bpe_encode_bytes_batch", "b200bpe_last_bytes_repairs", "b200bpe_last_miss_memo",
-    "b200bpe_encode_with_unstable_batch", "b200bpe_result_groups", "b200bpe_last_unstable",
+    "b200bpe_encode_with_unstable_batch", "b200bpe_result_groups", "b200bpe_last_unstable", "b200bpe_bpe_train",
 ]
 
 GREW_MISS, GREW_SLOW, GREW_LONG = 1, 2, 4       # B200BPE_GREW_* (b200bpe_last_reruns)
@@ -143,7 +145,7 @@ def check(rc: int) -> None:
     if rc == OK:
         return
     msg = last_error()
-    if rc in (EINVAL, EPATTERN, EDUPRANK, ESPECIAL):
+    if rc in (EINVAL, EPATTERN, EDUPRANK, ESPECIAL, ENOPAIR):
         raise ValueError(msg)
     if rc == EKEY:
         raise KeyError(msg)

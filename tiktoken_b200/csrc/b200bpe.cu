@@ -60,6 +60,7 @@
 #include "kernels_decode.cuh"
 #include "kernels_bytes.cuh"
 #include "kernels_unstable.cuh"
+#include "kernels_train.cuh"
 #include "unicode_classes.inc"
 
 using namespace b2bpe;
@@ -440,6 +441,11 @@ static void apply_l2_window(DevCtx *D, cudaStream_t st) {
     if (cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &v) != cudaSuccess) cudaGetLastError();
 }
 
+// the pre-tokeniser's class of every ASCII byte (its fast path), from the two-stage Unicode class tables
+static void uc_ascii_table(uint8_t *ascii) {
+    for (int i = 0; i < 128; i++) ascii[i] = UC_STAGE2[(uint32_t)UC_STAGE1[0] * 256 + i];
+}
+
 static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &boff, const std::vector<uint8_t> &blob,
                          DevCtx **out) {
     DevCtx *D = new DevCtx();
@@ -448,7 +454,7 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
     cudaError_t e = cudaSetDevice(device);
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&D->n_sm, cudaDevAttrMultiProcessorCount, device);
     uint8_t ascii[128];
-    for (int i = 0; i < 128; i++) ascii[i] = UC_STAGE2[(uint32_t)UC_STAGE1[0] * 256 + i];
+    uc_ascii_table(ascii);
     // one arena, hottest tables first: the L2 persistence window covers a prefix of it
     struct Part { const void *src; size_t bytes; size_t off; };
     enum { P_NARROW, P_WIDE, P_PAIR2, P_BYTE_ID, P_PAIR, P_ASCII, P_UC1, P_UC2, P_LONG, P_BLOB, N_PARTS };
@@ -1671,18 +1677,11 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     for (int i = 0; i < 3; i++) J->memo[i] += memo[i];
 }
 
-static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, bool single_piece,
-                       const uint8_t *sp_flags, b200bpe_result **out, int *special_idx, bool bytes = false,
-                       b200bpe_result **completions = nullptr) {
+// Chunk plan of the host path: document ranges [cut[c], cut[c+1]) of about `chunk` bytes each (a document larger than a
+// chunk is a chunk of its own); one chunk when the batch is at most 1.5 chunks or in single-piece mode.
+static int chunk_plan(const uint64_t *doc_off, uint64_t n_docs, size_t chunk, bool single_piece, std::vector<uint64_t> &cut) {
     const uint64_t n_bytes = doc_off[n_docs];
-    if (doc_off[0] != 0) return fail(B200BPE_EINVAL, "document offsets must start at 0");
-    const int n_dev = (int)h->devs.size();
-    if (!h->pool) h->pool = new TaskPool();
-    h->pool->ensure(h->copy_threads);
-    // ---- chunk plan: document ranges [lo, hi) ------------------------------------------------
-    size_t chunk = h->chunk_bytes;
-    if (!h->chunk_forced && n_dev > 1) chunk = std::min<size_t>(64u << 20, std::max<size_t>(8u << 20, (size_t)(n_bytes / (4 * (uint64_t)n_dev))));
-    std::vector<uint64_t> cut; cut.push_back(0);
+    cut.assign(1, 0);
     if (!single_piece && n_bytes > chunk + chunk / 2) {
         uint64_t lo = 0;
         while (lo < n_docs) {
@@ -1694,13 +1693,29 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
             cut.push_back(hi); lo = hi;
         }
     } else cut.push_back(n_docs);
-    const size_t n_chunks = cut.size() - 1;
-    for (size_t c = 0; c < n_chunks; c++) {
+    for (size_t c = 0; c + 1 < cut.size(); c++) {
         const uint64_t cb = doc_off[cut[c + 1]] - doc_off[cut[c]];
         if (doc_off[cut[c + 1]] < doc_off[cut[c]] || cb >= (1ull << 32) - 4096)
             return fail(B200BPE_EINVAL, cb >= (1ull << 32) - 4096 ? "a single document of >= 4 GiB is not supported"
                                                                   : "document offsets must be non-decreasing");
     }
+    return B200BPE_OK;
+}
+
+static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, bool single_piece,
+                       const uint8_t *sp_flags, b200bpe_result **out, int *special_idx, bool bytes = false,
+                       b200bpe_result **completions = nullptr) {
+    const uint64_t n_bytes = doc_off[n_docs];
+    if (doc_off[0] != 0) return fail(B200BPE_EINVAL, "document offsets must start at 0");
+    const int n_dev = (int)h->devs.size();
+    if (!h->pool) h->pool = new TaskPool();
+    h->pool->ensure(h->copy_threads);
+    // ---- chunk plan: document ranges [lo, hi) ------------------------------------------------
+    size_t chunk = h->chunk_bytes;
+    if (!h->chunk_forced && n_dev > 1) chunk = std::min<size_t>(64u << 20, std::max<size_t>(8u << 20, (size_t)(n_bytes / (4 * (uint64_t)n_dev))));
+    std::vector<uint64_t> cut;
+    if (int rc = chunk_plan(doc_off, n_docs, chunk, single_piece, cut)) return rc;
+    const size_t n_chunks = cut.size() - 1;
     bool pageable = false;
     if (n_bytes) {
         cudaPointerAttributes at;
@@ -2058,5 +2073,295 @@ extern "C" int b200bpe_last_unstable(b200bpe_t *h, uint64_t *stats5) {
 extern "C" int b200bpe_table_bytes(b200bpe_t *h, uint64_t *bytes4) {
     if (!h || !bytes4) return fail(B200BPE_EINVAL, "null argument");
     memcpy(bytes4, h->table_bytes, sizeof(h->table_bytes));
+    return B200BPE_OK;
+}
+
+// --------------------------------------------------------------------------------------------
+// BPE training (tiktoken/_educational.py:119-185 `bpe_train`), kernels_train.cuh
+// --------------------------------------------------------------------------------------------
+namespace {
+
+struct TrainRun {                              // everything one b200bpe_bpe_train call allocates on its device
+    DevBuf<uint8_t> all, ct, uc;
+    DevBuf<unsigned long long> doff, npieces, wkey, wcnt, wfirst, wused, part, tbase, dfirst, dcnt, woff;
+    DevBuf<unsigned long long> pkey, pcnt, th, tpw, tlen;
+    DevBuf<uint32_t> dbits, sfd, pbits, psum, slow, wlen, fbits, tcnt, dlen, wl1, sym, pocc, tslot, stamp, aff, merges;
+    Counters *ctr = nullptr, *h_ctr = nullptr; TrainState *st = nullptr, *h_st = nullptr;
+    unsigned long long *h_u64 = nullptr;
+    cudaStream_t s = nullptr;
+    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    cudaGraphExec_t exec = nullptr; cudaGraph_t graph = nullptr;
+    ~TrainRun() {
+        DevBuf<uint8_t> *b8[] = {&all, &ct, &uc};
+        for (auto *b : b8) b->release();
+        DevBuf<unsigned long long> *b64[] = {&doff, &npieces, &wkey, &wcnt, &wfirst, &wused, &part, &tbase, &dfirst, &dcnt, &woff,
+                                             &pkey, &pcnt, &th, &tpw, &tlen};
+        for (auto *b : b64) b->release();
+        DevBuf<uint32_t> *b32[] = {&dbits, &sfd, &pbits, &psum, &slow, &wlen, &fbits, &tcnt, &dlen, &wl1, &sym, &pocc, &tslot,
+                                   &stamp, &aff, &merges};
+        for (auto *b : b32) b->release();
+        if (ctr) cudaFree(ctr);
+        if (st) cudaFree(st);
+        if (h_ctr) cudaFreeHost(h_ctr);
+        if (h_st) cudaFreeHost(h_st);
+        if (h_u64) cudaFreeHost(h_u64);
+        if (exec) cudaGraphExecDestroy(exec);
+        if (graph) cudaGraphDestroy(graph);
+        for (auto &e : ev) if (e) cudaEventDestroy(e);
+        if (s) cudaStreamDestroy(s);
+    }
+};
+
+uint64_t train_pow2(uint64_t x) { uint64_t p = 1; while (p < x) p <<= 1; return p; }
+
+float event_ms(cudaEvent_t a, cudaEvent_t b) { float ms = 0.f; if (cudaEventElapsedTime(&ms, a, b) != cudaSuccess) { cudaGetLastError(); ms = 0.f; } return ms; }
+
+}  // namespace
+
+// make the piece table hold `need` slots at half load, keeping what it holds
+static int train_words_reserve(TrainRun &T, TrainWords &W, uint64_t need) {
+    const uint64_t want = train_pow2(std::max<uint64_t>(2 * need, 1u << 16));
+    if (W.key && W.mask + 1 >= want) return B200BPE_OK;
+    TrainRun O;                                           // the old table moves here and is freed on return
+    std::swap(O.wkey, T.wkey); std::swap(O.wcnt, T.wcnt); std::swap(O.wfirst, T.wfirst); std::swap(O.wlen, T.wlen);
+    const uint64_t n_old = W.key ? W.mask + 1 : 0;
+    CUDA_TRY(T.wkey.ensure(want)); CUDA_TRY(T.wcnt.ensure(want)); CUDA_TRY(T.wfirst.ensure(want)); CUDA_TRY(T.wlen.ensure(want));
+    CUDA_TRY(cudaMemsetAsync(T.wkey.p, 0, want * 8, T.s)); CUDA_TRY(cudaMemsetAsync(T.wcnt.p, 0, want * 8, T.s));
+    CUDA_TRY(cudaMemsetAsync(T.wfirst.p, 0xFF, want * 8, T.s));
+    TrainWords N{T.wkey.p, T.wcnt.p, T.wfirst.p, T.wlen.p, want - 1, T.wused.p};
+    if (n_old) {
+        CUDA_TRY(cudaMemsetAsync(T.wused.p, 0, 8, T.s));
+        TrainWords Wo{O.wkey.p, O.wcnt.p, O.wfirst.p, O.wlen.p, W.mask, W.n_used};
+        train_rehash_kernel<<<1024, 256, 0, T.s>>>(Wo, n_old, N);
+        CUDA_TRY(cudaStreamSynchronize(T.s));
+    }
+    W = N;
+    return B200BPE_OK;
+}
+
+extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, const char *pat_str,
+                                 uint32_t vocab_size, int device, uint32_t *merges_out, uint64_t merges_cap,
+                                 uint64_t *n_merges_out, double *stats8) {
+    if (stats8) for (int i = 0; i < 8; i++) stats8[i] = 0.0;
+    if (n_merges_out) *n_merges_out = 0;
+    if (!doc_off || !pat_str || !n_merges_out || (merges_cap && !merges_out)) return fail(B200BPE_EINVAL, "null argument");
+    int pattern;
+    if (strcmp(pat_str, R50K_PAT) == 0) pattern = PAT_R50K;
+    else if (strcmp(pat_str, CL100K_PAT) == 0) pattern = PAT_CL100K;
+    else if (strcmp(pat_str, O200K_PAT) == 0) pattern = PAT_O200K;
+    else return fail(B200BPE_EPATTERN, "unsupported pat_str: the GPU pre-tokeniser implements exactly the r50k/p50k, cl100k and "
+                                       "o200k patterns of tiktoken_ext/openai_public.py");
+    if (vocab_size < 256) return fail(B200BPE_EINVAL, "vocab_size must be at least 256, so we can encode all bytes");
+    if (doc_off[0] != 0) return fail(B200BPE_EINVAL, "document offsets must start at 0");
+    const uint64_t N = doc_off[n_docs];
+    if (N && !text) return fail(B200BPE_EINVAL, "null text");
+    size_t chunk = 64u << 20;
+    if (const char *cm = getenv("B200BPE_CHUNK_MB")) { long v = atol(cm); if (v >= 1 && v <= 2048) chunk = (size_t)v << 20; }
+    std::vector<uint64_t> cut;
+    if (int rc = chunk_plan(doc_off, n_docs, chunk, false, cut)) return rc;
+    const uint32_t target = vocab_size;
+    if (target == 256) return B200BPE_OK;                  // the 256 single bytes, no merge
+    if (merges_cap > 0xFFFFFFF0ull) merges_cap = 0xFFFFFFF0ull;
+    int ndev = 0;
+    if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0) { cudaGetLastError(); return fail(B200BPE_ECUDA, "no CUDA device: libb200bpe has no CPU fallback"); }
+    if (device < 0 || device >= ndev) return fail(B200BPE_EINVAL, "bad device index");
+    DeviceGuard guard;
+    CUDA_TRY(cudaSetDevice(device));
+    int n_sm = 0;
+    CUDA_TRY(cudaDeviceGetAttribute(&n_sm, cudaDevAttrMultiProcessorCount, device));
+    TrainRun T;
+    CUDA_TRY(cudaStreamCreateWithFlags(&T.s, cudaStreamNonBlocking));
+    for (auto &e : T.ev) CUDA_TRY(cudaEventCreate(&e));
+    CUDA_TRY(cudaMalloc((void **)&T.ctr, sizeof(Counters))); CUDA_TRY(cudaMalloc((void **)&T.st, sizeof(TrainState)));
+    CUDA_TRY(cudaHostAlloc((void **)&T.h_ctr, sizeof(Counters), cudaHostAllocPortable));
+    CUDA_TRY(cudaHostAlloc((void **)&T.h_st, sizeof(TrainState), cudaHostAllocPortable));
+    CUDA_TRY(cudaHostAlloc((void **)&T.h_u64, 4 * 8, cudaHostAllocPortable));
+    cudaStream_t s = T.s;
+    // Unicode class tables of the pre-tokeniser (the engine keeps them in its table arena)
+    UcTables uc;
+    {
+        uint8_t ascii[128];
+        uc_ascii_table(ascii);
+        const size_t o2 = (sizeof(UC_STAGE1) + 255) & ~(size_t)255, o3 = o2 + ((sizeof(UC_STAGE2) + 255) & ~(size_t)255);
+        CUDA_TRY(T.uc.ensure(o3 + 128));
+        CUDA_TRY(cudaMemcpy(T.uc.p, UC_STAGE1, sizeof(UC_STAGE1), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(T.uc.p + o2, UC_STAGE2, sizeof(UC_STAGE2), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(T.uc.p + o3, ascii, 128, cudaMemcpyHostToDevice));
+        uc.stage1 = (const uint16_t *)T.uc.p; uc.stage2 = T.uc.p + o2; uc.ascii = T.uc.p + o3; uc.one = 1u;
+    }
+    // the corpus stays on the device: each piece is compared with the first occurrence of its word
+    CUDA_TRY(T.all.ensure(N + 64));
+    if (N) CUDA_TRY(cudaMemcpy(T.all.p, text, N, cudaMemcpyHostToDevice));
+    CUDA_TRY(T.fbits.ensure((N + 1 + 1023) / 1024 * 32 + 64));
+    CUDA_TRY(cudaMemsetAsync(T.fbits.p, 0, T.fbits.cap * 4, s));
+    CUDA_TRY(cudaMemsetAsync(T.st, 0, sizeof(TrainState), s));
+    CUDA_TRY(T.npieces.ensure(1)); CUDA_TRY(T.wused.ensure(1));
+    CUDA_TRY(cudaMemsetAsync(T.wused.p, 0, 8, s));
+    TrainWords W{}; W.n_used = T.wused.p;
+    if (int rc = train_words_reserve(T, W, 1u << 15)) return rc;
+    double ms_split = 0, ms_words = 0, ms_loop = 0;
+    uint64_t n_pieces = 0;
+    // ---- split + distinct words, chunk by chunk --------------------------------------------------------------------
+    for (size_t c = 0; c + 1 < cut.size(); c++) {
+        const uint64_t lo = cut[c], hi = cut[c + 1], base = doc_off[lo], n = doc_off[hi] - base, nd = hi - lo;
+        if (n == 0) continue;
+        const long long n_words = (long long)((n + 1 + 31) / 32);
+        std::vector<unsigned long long> rel(nd + 1);
+        for (uint64_t d = 0; d <= nd; d++) rel[d] = doc_off[lo + d] - base;
+        CUDA_TRY(T.doff.ensure(nd + 1)); CUDA_TRY(T.ct.ensure(n + 64));
+        CUDA_TRY(T.dbits.ensure((size_t)n_words + 8)); CUDA_TRY(T.sfd.ensure((size_t)n_words + 4));
+        CUDA_TRY(T.pbits.ensure((size_t)n_words + 8)); CUDA_TRY(T.psum.ensure((size_t)(n_words >> 5) + 4));
+        CUDA_TRY(T.slow.ensure(n + 64));                   // every position: the slow list cannot overflow
+        CUDA_TRY(cudaMemcpyAsync(T.doff.p, rel.data(), (nd + 1) * 8, cudaMemcpyHostToDevice, s));
+        CUDA_TRY(cudaMemcpyAsync(T.ct.p, T.all.p + base, n, cudaMemcpyDeviceToDevice, s));   // 16-byte aligned chunk text
+        CUDA_TRY(cudaMemsetAsync(T.ct.p + n, 0, 64, s));
+        CUDA_TRY(cudaMemsetAsync(T.ctr, 0, sizeof(Counters), s));
+        CUDA_TRY(cudaMemsetAsync(T.dbits.p, 0, ((size_t)n_words + 8) * 4, s));
+        CUDA_TRY(cudaMemsetAsync(T.sfd.p, 0xFF, ((size_t)n_words + 4) * 4, s));
+        CUDA_TRY(cudaMemsetAsync(T.pbits.p + n_words, 0, 8 * 4, s));
+        CUDA_TRY(cudaMemsetAsync(T.npieces.p, 0, 8, s));
+        CUDA_TRY(cudaEventRecord(T.ev[0], s));
+        mark_docs_kernel<<<(unsigned)((nd + 1 + 255) / 256), 256, 0, s>>>(T.doff.p, nd, n, T.dbits.p, T.sfd.p, nullptr, T.ctr);
+        const unsigned grid = (unsigned)((n_words + 255) / 256);
+        const uint32_t scap = (uint32_t)std::min<uint64_t>(n + 64, 0xFFFFFFF0u);
+#define B2_TRAIN_PRETOK(P)                                                                                                  \
+    pretok_kernel<P><<<grid, 256, 0, s>>>(T.ct.p, (long long)n, T.dbits.p, uc, T.pbits.p, T.psum.p, n_words, nullptr,     \
+                                          T.slow.p, scap, T.ctr);                                                         \
+    pretok_slow_kernel<P><<<n_sm * 8, 256, 0, s>>>(T.ct.p, (long long)n, T.dbits.p, uc, T.pbits.p, T.psum.p, T.slow.p, scap, T.ctr)
+        if (pattern == PAT_R50K) { B2_TRAIN_PRETOK(PAT_R50K); }
+        else if (pattern == PAT_CL100K) { B2_TRAIN_PRETOK(PAT_CL100K); }
+        else { B2_TRAIN_PRETOK(PAT_O200K); }
+#undef B2_TRAIN_PRETOK
+        CUDA_TRY(cudaEventRecord(T.ev[1], s));
+        train_count_kernel<<<grid, 256, 0, s>>>(T.pbits.p, (long long)n, n_words, T.npieces.p);
+        CUDA_TRY(cudaMemcpyAsync(T.h_ctr, T.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(T.h_u64, T.npieces.p, 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaMemcpyAsync(T.h_u64 + 1, T.wused.p, 8, cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (T.h_ctr->err & ERR_DOCOFF) return fail(B200BPE_EINVAL, "malformed document offsets");
+        if (T.h_ctr->err) return fail(B200BPE_ECUDA, "pre-tokeniser error flags " + std::to_string(T.h_ctr->err));
+        n_pieces += T.h_u64[0];
+        ms_split += event_ms(T.ev[0], T.ev[1]);
+        if (int rc = train_words_reserve(T, W, T.h_u64[0] + T.h_u64[1])) return rc;
+        CUDA_TRY(cudaEventRecord(T.ev[2], s));
+        train_insert_kernel<<<grid, 256, 0, s>>>(T.ct.p, (long long)n, T.pbits.p, n_words, base, W);
+        train_verify_kernel<<<grid, 256, 0, s>>>(T.ct.p, (long long)n, T.pbits.p, n_words, base, W, T.all.p, T.fbits.p, T.st);
+        CUDA_TRY(cudaEventRecord(T.ev[3], s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        ms_words += event_ms(T.ev[2], T.ev[3]);
+    }
+    CUDA_TRY(cudaGetLastError());
+    // ---- words in order of first occurrence: CSR of symbol ids ----------------------------------------------------
+    CUDA_TRY(cudaEventRecord(T.ev[2], s));
+    const long long n_tiles = (long long)((N + 1 + 1023) / 1024);
+    CUDA_TRY(T.tcnt.ensure((size_t)n_tiles + 4)); CUDA_TRY(T.tbase.ensure((size_t)n_tiles + 4));
+    CUDA_TRY(T.part.ensure((size_t)(n_tiles / SCAN_ITEMS) + 4));
+    CUDA_TRY(cudaMemsetAsync(T.ctr, 0, sizeof(Counters), s));
+    train_tile_count_kernel<<<(unsigned)((n_tiles + 255) / 256), 256, 0, s>>>(T.fbits.p, n_tiles, T.tcnt.p);
+    {
+        const long long nb = (n_tiles + SCAN_ITEMS - 1) / SCAN_ITEMS;
+        scan_partial_kernel<<<(unsigned)nb, 256, 0, s>>>(T.tcnt.p, n_tiles, T.part.p);
+        scan_top_kernel<<<1, 1024, 0, s>>>(T.part.p, nb, T.ctr);
+        scan_final_kernel<<<(unsigned)nb, 256, 0, s>>>(T.tcnt.p, n_tiles, T.part.p, T.tbase.p, T.ctr);
+    }
+    CUDA_TRY(cudaMemcpyAsync(T.h_ctr, T.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(T.h_u64 + 1, T.wused.p, 8, cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    const uint64_t D = T.h_ctr->total_tokens;
+    if (D != T.h_u64[1]) return fail(B200BPE_ECUDA, "internal: distinct words and first occurrences disagree");
+    if (D >= 0xFFFFFFF0ull) return fail(B200BPE_EINVAL, "too many distinct words (>= 2^32)");
+    CUDA_TRY(T.dfirst.ensure(D + 2)); CUDA_TRY(T.dlen.ensure(D + 2)); CUDA_TRY(T.dcnt.ensure(D + 2)); CUDA_TRY(T.wl1.ensure(D + 2));
+    CUDA_TRY(T.woff.ensure(D + 2));
+    train_compact_kernel<<<n_sm * 8, 256, 0, s>>>(W, T.fbits.p, T.tbase.p, T.dfirst.p, T.dlen.p, T.dcnt.p, T.wl1.p, D, T.st);
+    {
+        const long long nb = ((long long)D + SCAN_ITEMS - 1) / SCAN_ITEMS;
+        CUDA_TRY(T.part.ensure((size_t)nb + 4));
+        CUDA_TRY(cudaMemsetAsync(T.ctr, 0, sizeof(Counters), s));
+        if (nb) {
+            scan_partial_kernel<<<(unsigned)nb, 256, 0, s>>>(T.wl1.p, (long long)D, T.part.p);
+            scan_top_kernel<<<1, 1024, 0, s>>>(T.part.p, nb, T.ctr);
+            scan_final_kernel<<<(unsigned)nb, 256, 0, s>>>(T.wl1.p, (long long)D, T.part.p, T.woff.p, T.ctr);
+        } else CUDA_TRY(cudaMemsetAsync(T.woff.p, 0, 8, s));
+    }
+    CUDA_TRY(cudaMemcpyAsync(T.h_ctr, T.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaMemcpyAsync(T.h_st, T.st, sizeof(TrainState), cudaMemcpyDeviceToHost, s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    if (T.h_st->err) return fail(B200BPE_ECUDA, T.h_st->err & 1u ? "internal: two different pieces share a 64-bit hash"
+                                                                 : "internal: word index out of range");
+    const uint64_t S = T.h_ctr->total_tokens;               // symbol slots: every word plus its separator
+    CUDA_TRY(T.sym.ensure(S + 4));
+    if (D) train_fill_kernel<<<n_sm * 8, 256, 0, s>>>(T.all.p, T.dfirst.p, T.dlen.p, T.woff.p, D, T.sym.p);
+    CUDA_TRY(cudaStreamSynchronize(s));
+    T.all.release(); T.ct.release(); T.slow.release(); T.pbits.release(); T.dbits.release(); T.sfd.release();
+    T.wkey.release(); T.wcnt.release(); T.wfirst.release(); T.wlen.release();
+    // pair table: distinct keys <= P0 initial pairs + 2 per merged occurrence (<= P0 in all) -> at most half full
+    const uint64_t P0 = S - 2 * D;
+    const uint64_t pcap = train_pow2(std::max<uint64_t>(6 * P0 + 1024, 1u << 12));
+    if (pcap > (1ull << 32)) return fail(B200BPE_EINVAL, "corpus too large for one training call (pair table >= 2^32 slots)");
+    CUDA_TRY(T.pkey.ensure(pcap)); CUDA_TRY(T.pcnt.ensure(pcap)); CUDA_TRY(T.pocc.ensure(pcap));
+    CUDA_TRY(cudaMemsetAsync(T.pkey.p, 0xFF, pcap * 8, s)); CUDA_TRY(cudaMemsetAsync(T.pcnt.p, 0, pcap * 8, s));
+    TrainPairs P{T.pkey.p, T.pcnt.p, T.pocc.p, pcap - 1};
+    const uint64_t tcap = train_pow2(2ull * target + 1024);
+    CUDA_TRY(T.th.ensure(target + 2)); CUDA_TRY(T.tpw.ensure(target + 2)); CUDA_TRY(T.tlen.ensure(target + 2));
+    CUDA_TRY(T.tslot.ensure(tcap));
+    CUDA_TRY(cudaMemsetAsync(T.tslot.p, 0xFF, tcap * 4, s));
+    TrainTok TT{T.th.p, T.tpw.p, T.tlen.p, T.tslot.p, tcap - 1};
+    train_tok_init_kernel<<<1, 32, 0, s>>>(TT);
+    CUDA_TRY(T.stamp.ensure(D + 2)); CUDA_TRY(T.aff.ensure(D + 2)); CUDA_TRY(T.merges.ensure(3 * merges_cap + 3));
+    CUDA_TRY(cudaMemsetAsync(T.stamp.p, 0, (D + 2) * 4, s));
+    {
+        TrainState init; memset(&init, 0, sizeof(init));
+        init.best = ~0ull; init.n_ids = 256;
+        *T.h_st = init;
+        CUDA_TRY(cudaMemcpyAsync(T.st, T.h_st, sizeof(TrainState), cudaMemcpyHostToDevice, s));
+    }
+    if (D) train_pairs_init_kernel<<<n_sm * 8, 256, 0, s>>>(T.sym.p, T.woff.p, T.dlen.p, T.dcnt.p, D, P, T.st);
+    CUDA_TRY(cudaEventRecord(T.ev[3], s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    CUDA_TRY(cudaGetLastError());
+    ms_words += event_ms(T.ev[2], T.ev[3]);
+    // ---- the merge loop: a CUDA graph of K steps, replayed until the state says stop ---------------------------------
+    const int K = (int)env_long("B200BPE_TRAIN_GRAPH_STEPS", 128, 1, 4096);
+    const unsigned mark_grid = (unsigned)std::min<uint64_t>((S + 255) / 256 + 1, (uint64_t)n_sm * 16);
+    CUDA_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
+    for (int k = 0; k < K; k++) {
+        train_max_kernel<<<n_sm * 4, 256, 0, s>>>(P, T.st);
+        train_first_kernel<<<n_sm * 4, 256, 0, s>>>(T.sym.p, S, P, T.st);
+        train_commit_kernel<<<1, 32, 0, s>>>(T.sym.p, TT, T.merges.p, (uint32_t)merges_cap, target, T.st);
+        train_mark_kernel<<<mark_grid, 256, 0, s>>>(T.sym.p, S, T.woff.p, D, T.stamp.p, T.aff.p, T.st);
+        train_apply_kernel<<<n_sm * 8, 256, 0, s>>>(T.sym.p, T.woff.p, T.dlen.p, T.dcnt.p, T.aff.p, P, T.st);
+    }
+    {
+        cudaError_t e = cudaStreamEndCapture(s, &T.graph);
+        if (e != cudaSuccess) return fail(B200BPE_ECUDA, std::string("graph capture: ") + cudaGetErrorString(e));
+    }
+    CUDA_TRY(cudaGraphInstantiate(&T.exec, T.graph, 0));
+    uint64_t batches = 0;
+    CUDA_TRY(cudaEventRecord(T.ev[0], s));
+    for (;;) {
+        CUDA_TRY(cudaGraphLaunch(T.exec, s));
+        batches++;
+        CUDA_TRY(cudaMemcpyAsync(T.h_st, T.st, sizeof(TrainState), cudaMemcpyDeviceToHost, s));
+        CUDA_TRY(cudaStreamSynchronize(s));
+        if (T.h_st->stop) break;
+    }
+    CUDA_TRY(cudaEventRecord(T.ev[1], s));
+    CUDA_TRY(cudaStreamSynchronize(s));
+    ms_loop = event_ms(T.ev[0], T.ev[1]);
+    const TrainState fin = *T.h_st;
+    if (fin.n_merges) CUDA_TRY(cudaMemcpy(merges_out, T.merges.p, (size_t)fin.n_merges * 12, cudaMemcpyDeviceToHost));
+    *n_merges_out = fin.n_merges;
+    if (stats8) {
+        stats8[0] = (double)n_pieces; stats8[1] = (double)D; stats8[2] = (double)fin.n_merges; stats8[3] = (double)batches;
+        stats8[4] = ms_split; stats8[5] = ms_words; stats8[6] = ms_loop; stats8[7] = (double)(cut.size() - 1);
+    }
+    if (fin.stop == TR_NOPAIR)
+        return fail(B200BPE_ENOPAIR, "no pair left to merge: the corpus allows " + std::to_string(fin.n_ids) +
+                                         " tokens, fewer than vocab_size = " + std::to_string(vocab_size));
+    if (fin.stop == TR_CAP)
+        return fail(B200BPE_ECAPACITY, "more than " + std::to_string(merges_cap) +
+                                           " merges: too many merges produced bytes that already were a token");
+    if (fin.stop != TR_DONE) return fail(B200BPE_ECUDA, "internal: training stopped with state " + std::to_string(fin.stop) +
+                                                         ", error bits " + std::to_string(fin.err));
     return B200BPE_OK;
 }
