@@ -137,8 +137,7 @@ int b200bpe_encode_with_unstable_batch(b200bpe_t *h, const uint8_t *text, const 
  * merges_out receives 3 uint32 per merge: left id, right id, merged id (ids 0..255 are the bytes; a new id is the number
  * of tokens so far); *n_merges_out their count.  At most merges_cap merges, else B200BPE_ECAPACITY.  No pair left
  * before vocab_size: B200BPE_ENOPAIR.  vocab_size < 256: B200BPE_EINVAL.  Runs on CUDA device `device`, the merge loop
- * without a host synchronisation per merge (a CUDA graph of B200BPE_TRAIN_GRAPH_STEPS merges, default 128, per host
- * check).  stats8 (may be NULL): [0] pieces, [1] distinct words, [2] merges, [3] graph batches, device ms of [4] the
+ * without a host synchronisation per merge (a CUDA graph of 128 merges per host check).  stats8 (may be NULL): [0] pieces, [1] distinct words, [2] merges, [3] graph batches, device ms of [4] the
  * split, [5] the distinct-word stage, [6] the merge loop, [7] chunks (B200BPE_CHUNK_MB, default 64 MiB). */
 int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, const char *pat_str,
                       uint32_t vocab_size, int device, uint32_t *merges_out, uint64_t merges_cap,

@@ -166,13 +166,11 @@ def test_missing_single_byte_raises_key_error():
     _check(e, o, text, off, 1)
 
 
-@pytest.mark.parametrize("pack", [0, 1])
-def test_chunk_seams(pack):
-    """1 MiB chunks: damaged documents on both sides of every seam, pinned and pageable input, with and without the
-    bit-packed token return."""
-    e, o, _ = _chunked_encoding("cl100k_base", 1, B200BPE_PACK=pack)
+def test_chunk_seams():
+    """1 MiB chunks: damaged documents on both sides of every seam, pinned and pageable input."""
+    e, o, _ = _chunked_encoding("cl100k_base", 1)
     o = BytesOracle(o, vu.load_encoding("cl100k_base", allow_real=False)[1])
-    rng = random.Random(9 + pack)
+    rng = random.Random(9)
     docs = _damage(_corpus_docs("cl100k_base", 7, 6 << 20, 60_000), rng, 0.5)
     docs += [b"\xff" + bytes(rng.randrange(256) for _ in range(300_000))]        # a 300 KB unstable piece in its own chunk
     text, off = _pack(docs)

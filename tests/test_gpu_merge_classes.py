@@ -13,7 +13,7 @@ import pytest
 
 import merge_class_inputs as mi
 import vocab_util as vu
-from test_gpu_paths import _chunked_encoding, _same
+from test_gpu_paths import _same
 
 pytestmark = pytest.mark.gpu
 CORES = os.cpu_count() or 1
@@ -144,18 +144,6 @@ def test_decode_returns_the_exact_bytes(layout):
     assert e.decode_bytes_batch([[ranks[longest]], [ranks[longest]] * 2]) == [longest, longest * 2]
     with pytest.raises(KeyError):
         e.decode_bytes_batch([[max(ranks.values()) + 3]])
-
-
-@pytest.mark.parametrize("layout", ["top_2p22m1", "top_2p22", "top_2p24m1", "top_2p24", "top_2p30m1"])
-def test_bit_packed_return(layout):
-    """B200BPE_PACK=1 in 1 MiB chunks: 22-, 23- and 24-bit fields; wider ids come back as plain u32."""
-    ranks = _ranks("base", layout)
-    special = mi.special_tokens(ranks)
-    e, o, _ = _chunked_encoding(f"merge_classes_pack_{layout}", 1, vocab=(vu.CL100K_PAT, ranks, special),
-                                B200BPE_PACK=1)
-    exp_t, exp_o = o.encode_ordinary_batch_np(TEXT, OFF, CORES)
-    assert _same(e.encode_ordinary_packed(TEXT, OFF), exp_t, exp_o)
-    _classes(e, CLS, ranks, "bit-packed return")
 
 
 def test_rank_limit():

@@ -149,10 +149,9 @@ def test_edge_keys_host_and_device_paths():
     _check_memo(e, _missed(o, ranks, docs[half:]), exact=True)
 
 
-@pytest.mark.parametrize("pack", [0, 1])
-def test_1mib_chunks(pack):
+def test_1mib_chunks():
     """Misses and merges summed over chunks; one memo per chunk, so a piece is merged once per chunk it occurs in."""
-    e, o, _ = _chunked_encoding("cl100k_base", 1, B200BPE_PACK=pack, B200BPE_MISS_MEMO_SLOTS=BIG_MEMO)
+    e, o, _ = _chunked_encoding("cl100k_base", 1, B200BPE_MISS_MEMO_SLOTS=BIG_MEMO)
     ranks = vu.load_encoding("cl100k_base", allow_real=False)[1]
     text, off = corpus.config2(nbytes=6 << 20, seed=31, doc_bytes=100_000)
     exp_t, exp_o = o.encode_ordinary_batch_np(text, off, CORES)

@@ -89,21 +89,6 @@ def test_chunk_seams_1mib_chunks(enc, kind):
     assert got == [o.encode(d, set(special)) for d in docs]
 
 
-@pytest.mark.parametrize("enc,kind", [("cl100k_base", corpus.ENGLISH), ("o200k_base", corpus.MIXED), ("r50k_base", corpus.CODE)])
-def test_bit_packed_token_return(enc, kind):
-    """B200BPE_PACK=1: tokens cross PCIe as 16..18-bit fields (pack_tokens_kernel) and helper threads widen them into the
-    result next to the pipeline -- many small chunks, pinned and pageable input, every token compared."""
-    e, o, _ = _chunked_encoding(enc, 1, B200BPE_PACK=1, B200BPE_COPY_THREADS=5)
-    text = corpus.generate(kind, 77, 9 << 20)
-    off = corpus.docs_fixed(text, 50_000, at_space=True)[1]
-    exp_t, exp_o = o.encode_ordinary_batch_np(text, off, CORES)
-    assert _same(e.encode_ordinary_packed(text, off), exp_t, exp_o)
-    assert _same(e.encode_ordinary_packed(text.copy(), off), exp_t, exp_o)
-    one = np.asarray([0, len(text)], np.uint64)                  # one document: one pipeline pass, one packed block
-    exp_t, exp_o = o.encode_ordinary_batch_np(text, one, CORES)
-    assert _same(e.encode_ordinary_packed(text, one), exp_t, exp_o)
-
-
 def test_default_chunks_over_200mib_full_compare():
     import tiktoken_b200
     pat, ranks, special, _ = vu.load_encoding("cl100k_base", allow_real=False)

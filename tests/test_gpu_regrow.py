@@ -111,24 +111,21 @@ def test_device_path_regrows(name):
     _three_calls(e, call, grown, passes)
 
 
-@pytest.mark.parametrize("variant", ["plain", "packed_return", "multi_gpu"])
+@pytest.mark.parametrize("variant", ["plain", "multi_gpu"])
 def test_batch_of_all_recipes_in_1mib_chunks(variant):
     """MISS, SLOW, LONG and TOKENS documents interleaved, 1 MiB chunks: every pipeline slot overflows on its first
     chunk while the other slots have uploads and kernels in flight, slots re-run with other causes later, and the
     whole batch overflows the pass-0 token buffer, so the second pass runs across all chunks (and devices).
-    Variants: as is; tokens returned bit-packed and widened by the unpacker thread (B200BPE_PACK=1); the one-process
-    multi-GPU engine."""
-    devices, env = None, {}
-    if variant == "packed_return":
-        env = {"B200BPE_PACK": 1}
-    elif variant == "multi_gpu":
+    Variants: as is; the one-process multi-GPU engine."""
+    devices = None
+    if variant == "multi_gpu":
         from tiktoken_b200 import _lib
         ndev = int(_lib.lib().b200bpe_device_count())
         if ndev < 2:
             pytest.skip("needs at least two CUDA devices")
         devices = list(range(min(ndev, 8)))
     text, off, kinds = ri.batch()
-    e, o, _ = _chunked_encoding("regrow_batch", 1, vocab=ri.vocabulary(ri.BATCH_VOCAB), devices=devices, **env)
+    e, o, _ = _chunked_encoding("regrow_batch", 1, vocab=ri.vocabulary(ri.BATCH_VOCAB), devices=devices)
     exp_t, exp_o = o.encode_ordinary_batch_np(text, off, CORES)
     assert len(exp_t) > ri.caps(len(text))["tokens"]
     # every document is one chunk (test_regrow_inputs.py checks that)

@@ -9,9 +9,11 @@
 //                         haystack boundaries, interior mask, special-piece mask + their ids
 //   pretok_kernel<PAT>    UTF-8 bytes + D -> piece-start bitmask P   (bit-parallel regex rules)
 //   find_long_kernel      P -> queue of pieces longer than 16 bytes + one work list per length class
-//   mid_thread_kernel     17..256 bytes: one piece per lane, 32 pieces per warp in one convergent
-//                         instruction stream, merge state in shared-memory columns
-//   long_piece_kernel     257..4096 bytes: a warp per piece;  giant_piece_kernel ..32768 bytes: a block per piece;
+//   mid_group{16,32}_kernel  17..128 bytes: a group of lanes per piece, merge state in shared memory
+//   pmerge{,_long}_kernel    129..1024 bytes: a warp per piece, a few rounds of parallel merges
+//                         (ranks of 2^22 and above: mid_thread_kernel 17..256 bytes, a piece per lane, and
+//                         long_piece_kernel 257..1024 bytes, a warp per piece)
+//   long_piece_kernel     1025..4096 bytes: a warp per piece;  giant_piece_kernel ..32768 bytes: a block per piece;
 //   cluster_piece_kernel  beyond: a thread-block cluster (8 x 1024 threads, DSMEM carries) per piece
 //                         -- the round-synchronous exact merge in global scratch
 //   probe_kernel          persistent warps, TMA-staged 1 KiB sub-tiles: whole-piece table probe of every short piece
@@ -121,8 +123,15 @@ long env_long(const char *name, long dflt, long lo, long hi) {
     return x < lo ? lo : x > hi ? hi : x;
 }
 
-// Persistent helper threads of one engine: they widen the bit-packed tokens that come back over PCIe and stage pageable
-// caller memory into pinned blocks, next to the device pipeline (the reference's counterpart is its rayon / thread pool).
+// B200BPE_CHUNK_MB: the host path's chunk size in MiB (1..2048), e.g. to place chunk seams in tests; 0 when unset
+size_t env_chunk_bytes() {
+    const char *v = getenv("B200BPE_CHUNK_MB");
+    const long x = v ? atol(v) : 0;
+    return x >= 1 && x <= 2048 ? (size_t)x << 20 : 0;
+}
+
+// Persistent helper threads of one engine: they stage pageable caller memory into pinned blocks, next to the device
+// pipeline (the reference's counterpart is its rayon / thread pool).
 struct TaskPool {
     std::vector<std::thread> th; std::mutex mu; std::condition_variable cv; std::deque<std::function<void()>> q; bool stop = false;
     void ensure(int n) {
@@ -161,15 +170,6 @@ void pool_for(TaskPool *pool, size_t n, size_t block, const std::function<void(s
     for (size_t b = 0; b < nb; b++) pool->push([&, b] { fn(b * block, std::min(n, (b + 1) * block)); latch.done(); });
     latch.wait();
 }
-// tokens come back from the device as `bits`-bit fields, little-endian bit order (pack_tokens_kernel); src is readable 8 bytes past the end
-void unpack_tokens(const uint8_t *src, uint32_t *dst, size_t lo, size_t hi, int bits) {
-    const uint64_t mask = (1ull << bits) - 1ull;
-    size_t bitpos = lo * (size_t)bits;
-    for (size_t i = lo; i < hi; i++, bitpos += (size_t)bits) {
-        uint64_t x; memcpy(&x, src + (bitpos >> 3), 8);
-        dst[i] = (uint32_t)((x >> (bitpos & 7)) & mask);
-    }
-}
 
 }  // namespace
 
@@ -201,13 +201,10 @@ struct Slot {
     cudaStream_t side = nullptr;     // the group kernels (17..1024 bytes) run here, next to probe + miss on the main stream,
     cudaStream_t side2 = nullptr;    // and the scratch kernels (warp / block / cluster per piece: a few SMs each) here
     cudaStream_t up = nullptr;       // host path: uploads of the slot's NEXT chunk (ordered behind the kernels, not the download, of its last one)
-    static const int N_EV = 16;       // [10] fork, [11] side start, [12] side end (join), [13] side2 end (join), [14] packed tokens on the host,
-                                      // [15] bytes mode: start of the tail runs
+    static const int N_EV = 15;       // [10] fork, [11] side start, [12] side end (join), [13] side2 end (join),
+                                      // [14] bytes mode: start of the tail runs
     cudaEvent_t ev[N_EV];
     PinnedBuf stage;                // pinned staging for callers whose text is pageable memory
-    DevBuf<uint32_t> w_pack;        // bit-packed tokens of the chunk (host path)
-    PinnedBuf stage_out;            // ... and where they land on the host before the helper threads widen them
-    std::atomic<int> stage_out_busy{0};
     float last_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
     uint32_t last_launches = 0;
     bool ok = false;
@@ -235,14 +232,12 @@ struct Slot {
         w_lq_start.release(); w_lq_off.release(); w_lq_len.release(); w_lq_ntok.release(); w_lq_cls.release(); w_big_n.release();
         w_sort_hist.release(); w_big_dst.release(); w_big_src.release(); w_scan_part.release();
         w_idA.release(); w_rkA.release(); w_idB.release(); w_rkB.release(); w_aux1.release(); w_aux2.release();
-        w_flag.release(); w_pack.release();
+        w_flag.release();
         w_vup.release(); w_kdrop.release(); w_btail.release(); w_b2out.release(); w_bout.release(); w_btext.release();
         w_b2doc.release(); w_b2off.release(); w_bbase.release(); w_bpart.release();
         w_ulen.release(); w_unit.release();
         if (stage.p) cudaFreeHost(stage.p);
         stage.p = nullptr; stage.cap = 0;
-        if (stage_out.p) cudaFreeHost(stage_out.p);
-        stage_out.p = nullptr; stage_out.cap = 0;
         long_cap = miss_cap = mres_cap = slow_cap = 0;
     }
     void destroy() {
@@ -283,13 +278,10 @@ struct UnstWs {
     }
 };
 
-#ifndef B2_N_SLOTS
-#define B2_N_SLOTS 3          // pipeline slots per device: uploads run B2_N_SLOTS - 2 chunks ahead of the kernels
-#endif
 // Everything that lives on one CUDA device: the replicated tables and the pipeline slots.
 struct DevCtx {
     int device = 0;
-    uint8_t *arena = nullptr; size_t arena_bytes = 0, hot_bytes = 0;   // all tables in one allocation (one L2 window)
+    uint8_t *arena = nullptr; size_t arena_bytes = 0;                  // all tables in one allocation
     DevTables T; UcTables uc;
     uint32_t *d_tok_boff = nullptr; uint8_t *d_tok_blob = nullptr;     // decode: id -> bytes
     uint32_t *d_tok_space = nullptr;                                   // bit per id: every byte is ' ', '\n' or '\t' (uploaded by
@@ -299,11 +291,9 @@ struct DevCtx {
     UnstTables ut;                                                     // completion search tables (the first such call)
     uint8_t *d_ut_arena = nullptr;
     UnstWs uw;                                                         // completion search work-space (one chunk at a time)
-    static const int N_SLOTS = B2_N_SLOTS;
-    Slot slots[B2_N_SLOTS];
-    size_t l2_window = 0; float l2_ratio = 0.f;
+    static const int N_SLOTS = 3;     // pipeline slots per device: uploads run N_SLOTS - 2 chunks ahead of the kernels
+    Slot slots[N_SLOTS];
     int n_sm = 0;                     // multiprocessors: the persistent and work-queue kernels launch a multiple of this
-    int probe_blocks_per_sm = 12;
 };
 
 struct b200bpe_result {
@@ -370,11 +360,8 @@ struct b200bpe {
     size_t chunk_bytes = 64u << 20; bool chunk_forced = false;
     int copy_threads = 4;
     TaskPool *pool = nullptr;        // helper threads (created with the first host-path call)
-    int pack_bits = 0;               // host path: tokens cross PCIe as fields of this many bits (0: plain u32)
     long memo_slots = -1;            // miss memo slots per call: -1 from the batch size, 0 off (B200BPE_MISS_MEMO_SLOTS)
-    bool mid_group = true;           // 17..1024-byte pieces: group-of-lanes kernels (need ranks < 2^22)
-    bool pmerge = true;              // 129..1024-byte pieces: segmented parallel merge (needs ranks < 2^22); off: the group-of-lanes kernels
-    int pmerge_min_cls = 3;          // shortest length class the parallel merge takes (3: 129..256 bytes; 0: everything from 17 bytes)
+    bool mid_group = true;           // 17..1024-byte pieces: group-of-lanes and parallel-merge kernels (need ranks < 2^22)
     std::mutex mu;
     std::vector<PinnedBuf> pinned_pool;
     // results keep the engine alive: b200bpe_destroy with results outstanding only marks the handle dead, the last
@@ -429,18 +416,6 @@ static void devctx_destroy(DevCtx *D) {
     delete D;
 }
 
-static void apply_l2_window(DevCtx *D, cudaStream_t st) {
-    if (!D->l2_window) return;
-    cudaStreamAttrValue v;
-    memset(&v, 0, sizeof(v));
-    v.accessPolicyWindow.base_ptr = D->arena;
-    v.accessPolicyWindow.num_bytes = D->l2_window;
-    v.accessPolicyWindow.hitRatio = D->l2_ratio;
-    v.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
-    v.accessPolicyWindow.missProp = cudaAccessPropertyStreaming;
-    if (cudaStreamSetAttribute(st, cudaStreamAttributeAccessPolicyWindow, &v) != cudaSuccess) cudaGetLastError();
-}
-
 // the pre-tokeniser's class of every ASCII byte (its fast path), from the two-stage Unicode class tables
 static void uc_ascii_table(uint8_t *ascii) {
     for (int i = 0; i < 128; i++) ascii[i] = UC_STAGE2[(uint32_t)UC_STAGE1[0] * 256 + i];
@@ -455,7 +430,7 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
     if (e == cudaSuccess) e = cudaDeviceGetAttribute(&D->n_sm, cudaDevAttrMultiProcessorCount, device);
     uint8_t ascii[128];
     uc_ascii_table(ascii);
-    // one arena, hottest tables first: the L2 persistence window covers a prefix of it
+    // one arena, hottest tables first
     struct Part { const void *src; size_t bytes; size_t off; };
     enum { P_NARROW, P_WIDE, P_PAIR2, P_BYTE_ID, P_PAIR, P_ASCII, P_UC1, P_UC2, P_LONG, P_BLOB, N_PARTS };
     Part parts[N_PARTS] = {{H.narrow_tab.data(), H.narrow_tab.size() * sizeof(U4), 0},
@@ -465,7 +440,7 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
                            {H.long_tab.data(), H.long_tab.size() * sizeof(U4), 0}, {H.long_blob.data(), H.long_blob.size(), 0}};
     size_t total = 0;
     for (auto &p : parts) { p.off = total; total += (p.bytes + 255) & ~(size_t)255; }
-    D->arena_bytes = total; D->hot_bytes = parts[P_ASCII].off;
+    D->arena_bytes = total;
     if (e == cudaSuccess) e = cudaMalloc((void **)&D->arena, total);
     for (auto &p : parts) if (e == cudaSuccess && p.bytes) e = cudaMemcpy(D->arena + p.off, p.src, p.bytes, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMalloc((void **)&D->d_tok_boff, boff.size() * 4);
@@ -475,16 +450,6 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
     if (e == cudaSuccess) e = special_upload(h->sp_host, &D->d_sp_arena, &D->sp);
     for (int i = 0; i < DevCtx::N_SLOTS && e == cudaSuccess; i++) e = D->slots[i].init();
     if (e == cudaSuccess) e = cudaFuncSetAttribute(mid_thread_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)MID_SMEM_BYTES);
-    if (e == cudaSuccess) {
-        const long carve = env_long("B200BPE_PROBE_CARVEOUT", -1, -1, 100);
-        if (carve >= 0) e = cudaFuncSetAttribute(probe_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)carve);
-        const long mcarve = env_long("B200BPE_MISS_CARVEOUT", -1, -1, 100);
-        if (e == cudaSuccess && mcarve >= 0) e = cudaFuncSetAttribute(miss_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, (int)mcarve);
-        // 12 blocks per SM where 10 fit at once: a block's share of the strided sub-tiles is smaller, and blocks that
-        // do not fit yet start as others finish.  Measured on an H100 80GB HBM3 at 700 W, config 2: probe_kernel 3.2
-        // ms with 10, 3.0 with 12, 3.4 with 16 (DESIGN §9)
-        D->probe_blocks_per_sm = (int)env_long("B200BPE_PROBE_BLOCKS", 12, 1, 16);
-    }
     if (e != cudaSuccess) { std::string m = cudaGetErrorString(e); devctx_destroy(D); return fail(B200BPE_ECUDA, "device " + std::to_string(device) + " setup: " + m); }
     D->T.narrow_tab = (const U4 *)(D->arena + parts[P_NARROW].off); D->T.narrow_mask = H.narrow_mask;
     D->T.wide_tab = (const U4 *)(D->arena + parts[P_WIDE].off); D->T.wide_mask = H.wide_mask;
@@ -498,23 +463,6 @@ static int devctx_create(b200bpe *h, int device, const std::vector<uint32_t> &bo
     D->T.long_tab = (const U4 *)(D->arena + parts[P_LONG].off); D->T.long_mask = H.long_mask;
     D->T.long_blob = D->arena + parts[P_BLOB].off;
     D->T.max_token_len = H.max_token_len; D->T.n_long_tokens = H.n_long_tokens;
-    // L2 persistence (off by default): a persisting access-policy window over the rank tables was measured on an H100
-    // 80GB HBM3 (SXM, 700 W power limit) at 1 GiB per step -- cl100k English 120.8 GB/s without the window vs 64.6 with
-    // it, o200k mixed scripts 23.9 vs 19.2: the set-aside costs the streams far more than it saves the table probes.
-    // B200BPE_L2_PERSIST=1 turns it on for experiments.
-    if (env_long("B200BPE_L2_PERSIST", 0, 0, 1)) {
-        int max_win = 0, max_persist = 0;
-        cudaDeviceGetAttribute(&max_win, cudaDevAttrMaxAccessPolicyWindowSize, device);
-        cudaDeviceGetAttribute(&max_persist, cudaDevAttrMaxPersistingL2CacheSize, device);
-        if (max_win > 0 && max_persist > 0) {
-            const size_t want = std::min((size_t)max_persist, D->hot_bytes);
-            if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) == cudaSuccess) {
-                D->l2_window = std::min(D->hot_bytes, (size_t)max_win);
-                D->l2_ratio = (float)std::min(1.0, (double)want / (double)D->l2_window);
-            } else cudaGetLastError();
-        }
-    }
-    for (int i = 0; i < DevCtx::N_SLOTS; i++) apply_l2_window(D, D->slots[i].stream);
     *out = D;
     return B200BPE_OK;
 }
@@ -548,7 +496,7 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
     DeviceGuard guard;
     b200bpe *h = new b200bpe();
     h->pattern = pattern;
-    int rc = build_tables(tok_bytes, tok_off, tok_rank, n_tok, h->H, (uint32_t)env_long("B200BPE_PAIR_SLACK", 3, 2, 16));
+    int rc = build_tables(tok_bytes, tok_off, tok_rank, n_tok, h->H);
     if (rc) { std::string m = h->H.error; delete h; return fail(rc == -3 ? B200BPE_EDUPRANK : B200BPE_EINVAL, m); }
     for (uint32_t i = 0; i < n_sp; i++) {
         std::string s((const char *)sp_bytes + sp_off[i], (size_t)(sp_off[i + 1] - sp_off[i]));
@@ -588,21 +536,10 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
         if (rc) { for (auto *d : h->devs) devctx_destroy(d); delete h; return rc; }
         h->devs.push_back(D);
     }
-    if (const char *cm = getenv("B200BPE_CHUNK_MB")) { long v = atol(cm); if (v >= 1 && v <= 2048) { h->chunk_bytes = (size_t)v << 20; h->chunk_forced = true; } }
-    h->mid_group = H.max_rank < MIDG_MAX_RANK && env_long("B200BPE_MID_GROUP", 1, 0, 1) != 0;
-    h->pmerge = h->mid_group && env_long("B200BPE_PMERGE", 1, 0, 1) != 0;
-    h->pmerge_min_cls = (int)env_long("B200BPE_PMERGE_MIN_CLS", 3, 1, 3);
+    if (const size_t cb = env_chunk_bytes()) { h->chunk_bytes = cb; h->chunk_forced = true; }
+    h->mid_group = H.max_rank < MIDG_MAX_RANK;
     h->memo_slots = env_long("B200BPE_MISS_MEMO_SLOTS", -1, 0, 1l << 24);
     h->copy_threads = (int)env_long("B200BPE_COPY_THREADS", std::max(1u, std::min(16u, std::thread::hardware_concurrency() / 4)), 1, 64);
-    {   // tokens return over PCIe as bit fields just wide enough for the largest id (17 bits for cl100k, 18 for o200k, 16 for
-        // r50k / p50k instead of 32): the return traffic shares the link with the text going up
-        uint32_t max_id = H.max_rank;
-        for (uint32_t r : h->special_rank) max_id = std::max(max_id, r);
-        int bits = 1;
-        while (bits < 32 && (max_id >> bits)) bits++;
-        bits = std::max(bits, 8);
-        h->pack_bits = (bits <= 24 && env_long("B200BPE_PACK", 0, 0, 1)) ? bits : 0;   // opt-in: see DESIGN 4
-    }
     h->table_bytes[0] = (H.narrow_tab.size() + H.wide_tab.size()) * sizeof(U4);
     h->table_bytes[1] = H.pair_tab.size() * sizeof(U4) + 65536 * 4 + 1024;
     h->table_bytes[2] = H.long_tab.size() * sizeof(U4) + H.long_blob.size();
@@ -837,15 +774,10 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         CUDA_TRY(cudaStreamWaitEvent(ls2, S.ev[10], 0));
         CUDA_TRY(cudaEventRecord(S.ev[11], ls));
         LongScratch LS{S.w_idA.p, S.w_rkA.p, S.w_idB.p, S.w_rkB.p, S.w_aux1.p, S.w_aux2.p, S.w_flag.p};
-        if (h->pmerge) {         // 129..1024 bytes: segmented parallel merge (rounds, not merges, are sequential); shorter: a group of lanes per piece
+        if (h->mid_group) {      // 129..1024 bytes: segmented parallel merge (rounds, not merges, are sequential); shorter: a group of lanes per piece
             pmerge_kernel<256, 3><<<D->n_sm * 10, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
             pmerge_long_kernel<<<D->n_sm * 4, PM_WARPS_L * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            if (h->pmerge_min_cls <= 2) pmerge_kernel<128, 2><<<D->n_sm * 16, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            else mid_group32_kernel<<<D->n_sm * 4, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 2);
-            if (h->pmerge_min_cls <= 1) pmerge_kernel<64, 1><<<D->n_sm * 16, PM_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
-            mid_group16_kernel<<<D->n_sm * 9, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, h->pmerge_min_cls <= 1 ? 0 : 1);
-        } else if (h->mid_group) {      // 17..1024 bytes: a group of lanes per piece, state in shared memory
-            mid_group32_kernel<<<D->n_sm * 4, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 4);
+            mid_group32_kernel<<<D->n_sm * 4, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 2);
             mid_group16_kernel<<<D->n_sm * 9, MIDG_WARPS * 32, 0, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr, 1);
         } else {                 // ranks of 2^22 and above: one piece per lane (72 KiB of columns per block) / warp per piece
             mid_thread_kernel<<<D->n_sm * 3, MID_WARPS * 32, MID_SMEM_BYTES, ls>>>(a.d_text, D->T, q, S.w_ltok.p, S.d_ctr);
@@ -877,7 +809,7 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         memo.block_n = S.w_memo_bn.p; memo.mask = memo_slots ? memo_slots - 1 : 0; memo.on = memo_slots ? 1u : 0u;
         memo.limit = std::max<uint32_t>(1u, memo_slots / 2 / (uint32_t)(D->n_sm * SORT_BLOCKS_PER_SM));   // per dedup block
         const long long want_blocks = (n_tiles + ENC_WARPS - 1) / ENC_WARPS;
-        const unsigned probe_grid = (unsigned)std::min<long long>(want_blocks, (long long)D->n_sm * D->probe_blocks_per_sm);
+        const unsigned probe_grid = (unsigned)std::min<long long>(want_blocks, (long long)D->n_sm * PROBE_BLOCKS_PER_SM);
         probe_kernel<<<probe_grid, ENC_WARPS * 32, 0, st>>>(p, D->T);
         CUDA_TRY(cudaEventRecord(S.ev[8], st));
         const int sort_blocks = D->n_sm * SORT_BLOCKS_PER_SM;
@@ -986,7 +918,6 @@ static int device_enqueue_locked(b200bpe *h, const PendingDeviceCall &c) {
     DevCtx *D = h->devs[0];
     Slot &S = D->slots[0];
     cudaStream_t st = c.st ? c.st : S.stream;
-    if (c.st) apply_l2_window(D, st);
     const uint8_t *txt = c.d_text;
     if (((uintptr_t)c.d_text & 15u) != 0) {                       // TMA staging and vector loads need 16-byte alignment
         CUDA_TRY(S.w_text.ensure((size_t)c.n_bytes + 64));
@@ -1126,7 +1057,7 @@ static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, u
     CUDA_TRY(S.w_bpart.ensure((size_t)(nd / SCAN_ITEMS) + 4));
     CUDA_TRY(S.w_btext.ensure((size_t)tail + 64)); CUDA_TRY(S.w_b2out.ensure((size_t)tail + 64));
     if (!S.d_bctr) CUDA_TRY(cudaMalloc((void **)&S.d_bctr, sizeof(Counters)));
-    CUDA_TRY(cudaEventRecord(S.ev[15], st));
+    CUDA_TRY(cudaEventRecord(S.ev[14], st));
     enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_b2doc.p, S.d_bctr, st);
     bytes_gather_kernel<<<(unsigned)((tail + 16 * 256 - 1) / (16 * 256)), 256, 0, st>>>(a1.d_text, nd, S.w_vup.p, S.w_b2doc.p, S.w_btext.p);
     PipeArgs a2;
@@ -1134,7 +1065,7 @@ static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, u
     a2.d_out = S.w_b2out.p; a2.d_tok_off = S.w_b2off.p; a2.st = st; a2.single_piece = true;
     int rc = run_again(h, D, S, a2, cls, memo, grown, reruns);
     if (rc) return rc;
-    float ms2 = 0; cudaEventElapsedTime(&ms2, S.ev[15], S.ev[4]);
+    float ms2 = 0; cudaEventElapsedTime(&ms2, S.ev[14], S.ev[4]);
     const uint32_t launches2 = S.last_launches;
     *nt = n1 - drop + S.h_ctr->total_tokens;
     CUDA_TRY(S.w_bout.ensure((size_t)std::max<uint64_t>(*nt, a1.n_bytes) + 64));
@@ -1484,42 +1415,13 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     const size_t n_chunks = J->cut.size() - 1;
     std::vector<size_t> mine;
     for (size_t c = first; c < n_chunks; c += step) mine.push_back(c);
-    // ---- packed return path: a thread of its own waits for the packed tokens of a chunk to land in pinned staging and has
-    //      the pool widen them into the result, so that neither the device pipeline nor this worker waits for host memory
-    struct UnpackJob { Slot *S; cudaEvent_t ev; const uint8_t *src; uint32_t *dst; uint64_t n; };
-    std::mutex uq_mu; std::condition_variable uq_cv; std::deque<UnpackJob> uq; bool uq_stop = false;
-    const int pack_bits = (h->pack_bits && !J->single_piece) ? h->pack_bits : 0;
-    std::thread unpacker;
-    auto stop_unpacker = [&] {
-        if (!unpacker.joinable()) return;
-        { std::lock_guard<std::mutex> lk(uq_mu); uq_stop = true; }
-        uq_cv.notify_all();
-        unpacker.join();                                         // drains the queue first
-    };
     auto bail = [&](int rc) {
         if (rc) J->set_error(rc);
         for (size_t k = 0; k < mine.size(); k++) { long long m1 = -1; J->count[mine[k]].compare_exchange_strong(m1, 0); }   // never leave a waiter spinning
         for (int i = 0; i < DevCtx::N_SLOTS; i++) { cudaStreamSynchronize(D->slots[i].up); cudaStreamSynchronize(D->slots[i].stream); }
-        stop_unpacker();                                         // after the copies: everything queued is widened before we return
     };
     if (mine.empty()) return;
     if (cudaSetDevice(D->device) != cudaSuccess) { fail(B200BPE_ECUDA, "cudaSetDevice failed"); return bail(B200BPE_ECUDA); }
-    if (pack_bits) unpacker = std::thread([&] {
-        cudaSetDevice(D->device);
-        for (;;) {
-            UnpackJob job;
-            {
-                std::unique_lock<std::mutex> lk(uq_mu);
-                uq_cv.wait(lk, [&] { return uq_stop || !uq.empty(); });
-                if (uq.empty()) return;
-                job = uq.front(); uq.pop_front();
-            }
-            if (cudaEventSynchronize(job.ev) == cudaSuccess)
-                pool_for(h->pool, (size_t)job.n, (size_t)1 << 19, [&](size_t lo, size_t hi) { unpack_tokens(job.src, job.dst, lo, hi, pack_bits); });
-            else J->set_error(fail(B200BPE_ECUDA, "cudaEventSynchronize failed in the token unpacker"));
-            job.S->stage_out_busy.store(0);
-        }
-    });
     const uint64_t *doc_off = J->doc_off;
     auto slot_of = [&](size_t k) -> Slot & { return D->slots[k % DevCtx::N_SLOTS]; };
 
@@ -1624,25 +1526,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         if (token_base) add_offset_kernel<<<(unsigned)((nd + 1 + 255) / 256), 256, 0, S.stream>>>(S.w_tokoff.p, nd + 1, (long long)token_base);
         CUDA_TRY(cudaEventRecord(S.ev[5], S.stream));
         CUDA_TRY(cudaMemcpyAsync((uint64_t *)J->r->off.p + lo, S.w_tokoff.p, (nd + 1) * 8, cudaMemcpyDeviceToHost, S.stream));
-        if (nt && pack_bits) {
-            const unsigned long long n_words = (nt * (uint64_t)pack_bits + 31) / 32;
-            const size_t bytes = (size_t)n_words * 4;
-            CUDA_TRY(S.w_pack.ensure((size_t)n_words + 4));
-            while (S.stage_out_busy.load()) std::this_thread::yield();        // the slot's previous chunk is still being widened
-            if (S.stage_out.cap < bytes + 16) {
-                if (S.stage_out.p) cudaFreeHost(S.stage_out.p);
-                S.stage_out.p = nullptr; S.stage_out.cap = 0;
-                const size_t want = bytes + bytes / 4 + 4096;
-                CUDA_TRY(cudaHostAlloc(&S.stage_out.p, want, cudaHostAllocPortable));
-                S.stage_out.cap = want;
-            }
-            pack_tokens_kernel<<<(unsigned)((n_words + 255) / 256), 256, 0, S.stream>>>(S.w_out.p, nt, pack_bits, S.w_pack.p, n_words);
-            CUDA_TRY(cudaMemcpyAsync(S.stage_out.p, S.w_pack.p, bytes, cudaMemcpyDeviceToHost, S.stream));
-            CUDA_TRY(cudaEventRecord(S.ev[14], S.stream));
-            S.stage_out_busy.store(1);
-            { std::lock_guard<std::mutex> lk(uq_mu); uq.push_back({&S, S.ev[14], (const uint8_t *)S.stage_out.p, (uint32_t *)J->r->tok.p + token_base, nt}); }
-            uq_cv.notify_one();
-        } else if (nt) CUDA_TRY(cudaMemcpyAsync((uint32_t *)J->r->tok.p + token_base, S.w_out.p, nt * 4, cudaMemcpyDeviceToHost, S.stream));
+        if (nt) CUDA_TRY(cudaMemcpyAsync((uint32_t *)J->r->tok.p + token_base, S.w_out.p, nt * 4, cudaMemcpyDeviceToHost, S.stream));
         CUDA_TRY(cudaEventRecord(S.ev[6], S.stream));
         for (int i = 0; i < 5; i++) sum_ms[i] += S.last_ms[i];
         sum_ms[7] += S.last_ms[7]; sum_ms[8] += S.last_ms[8]; sum_ms[5] += h2d; launches += S.last_launches;
@@ -2155,8 +2039,8 @@ extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, u
     if (doc_off[0] != 0) return fail(B200BPE_EINVAL, "document offsets must start at 0");
     const uint64_t N = doc_off[n_docs];
     if (N && !text) return fail(B200BPE_EINVAL, "null text");
-    size_t chunk = 64u << 20;
-    if (const char *cm = getenv("B200BPE_CHUNK_MB")) { long v = atol(cm); if (v >= 1 && v <= 2048) chunk = (size_t)v << 20; }
+    size_t chunk = env_chunk_bytes();
+    if (!chunk) chunk = 64u << 20;
     std::vector<uint64_t> cut;
     if (int rc = chunk_plan(doc_off, n_docs, chunk, false, cut)) return rc;
     const uint32_t target = vocab_size;
@@ -2321,7 +2205,7 @@ extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, u
     CUDA_TRY(cudaGetLastError());
     ms_words += event_ms(T.ev[2], T.ev[3]);
     // ---- the merge loop: a CUDA graph of K steps, replayed until the state says stop ---------------------------------
-    const int K = (int)env_long("B200BPE_TRAIN_GRAPH_STEPS", 128, 1, 4096);
+    const int K = 128;
     const unsigned mark_grid = (unsigned)std::min<uint64_t>((S + 255) / 256 + 1, (uint64_t)n_sm * 16);
     CUDA_TRY(cudaStreamBeginCapture(s, cudaStreamCaptureModeThreadLocal));
     for (int k = 0; k < K; k++) {

@@ -61,7 +61,7 @@ inline uint64_t long_hash_bytes(const uint8_t *p, uint32_t len) {
 
 // returns 0 or a negative B200BPE_E* code (values mirrored from include/b200bpe.h)
 inline int build_tables(const uint8_t *tok_bytes, const uint64_t *tok_off, const uint32_t *tok_rank,
-                        uint32_t n, HostTables &H, uint32_t pair_slack = 3) {
+                        uint32_t n, HostTables &H) {
     std::unordered_map<std::string, uint32_t> enc;
     enc.reserve((size_t)n * 2 + 16);
     H.decoder.reserve((size_t)n * 2 + 16);
@@ -110,10 +110,10 @@ inline int build_tables(const uint8_t *tok_bytes, const uint64_t *tok_off, const
     std::sort(pairs.begin(), pairs.end(), [](const Pair &x, const Pair &y) {
         return x.r != y.r ? x.r < y.r : x.a != y.a ? x.a < y.a : x.b < y.b;
     });
-    // linear probing over single slots; capacity >= pair_slack x the entries (load <= 1/3 by default).  Word w of a slot
+    // linear probing over single slots; capacity >= 3 x the entries (load <= 1/3).  Word w of a slot
     // is 1 when the probe path of some key passes through it (the key lives further on): a slot without that mark that
     // does not hold the key ends the chain, so an absent pair usually costs one load even when its home slot is taken.
-    uint32_t nslots = pow2_at_least((uint64_t)pairs.size() * pair_slack + 2);
+    uint32_t nslots = pow2_at_least((uint64_t)pairs.size() * 3 + 2);
     H.pair_mask = nslots - 1;
     H.pair_tab.assign((size_t)nslots, U4{PAIR_EMPTY, PAIR_EMPTY, RANK_MAX, 0});
     for (auto &p : pairs) {

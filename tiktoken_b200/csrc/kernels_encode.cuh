@@ -67,6 +67,10 @@ struct TileParams {
 };
 
 static const int ENC_WARPS = 4;                          // warps per block
+// probe_kernel grid: 12 blocks per SM where 10 fit at once, so a block's share of the strided sub-tiles is smaller and
+// blocks that do not fit yet start as others finish.  Measured on an H100 80GB HBM3 at 700 W, config 2: probe_kernel
+// 3.2 ms with 10, 3.0 with 12, 3.4 with 16 (DESIGN §9)
+static const int PROBE_BLOCKS_PER_SM = 12;
 static const int SUB_BYTES = 1024;                       // bytes per warp sub-tile (also: max pieces per sub-tile)
 static const int STAGE_TEXT = SUB_BYTES + 32;            // staged text: the sub-tile + 32 bytes of look-ahead
 static const int STAGE_PW = 36;                          // staged piece-start words: 32 own + 2 look-ahead (+2: 16-byte multiple)
@@ -607,19 +611,4 @@ __global__ void __launch_bounds__(256) big_copy_kernel(TileParams p) {
         for (unsigned long long x = blockIdx.x * 256ull + threadIdx.x; x < n; x += (unsigned long long)gridDim.x * 256ull)
             p.out[dst + x] = p.ltok[src + x];
     }
-}
-
-// host path: tokens -> fields of `bits` bits, little-endian bit order (token i occupies bits [i*bits, (i+1)*bits) of the
-// stream); one output word per thread, assembled from the 2..5 tokens that overlap it.  Halves the PCIe return traffic.
-__global__ void __launch_bounds__(256) pack_tokens_kernel(const uint32_t *__restrict__ tok, unsigned long long n, int bits,
-                                                         uint32_t *__restrict__ out, unsigned long long n_words) {
-    const unsigned long long w = blockIdx.x * 256ull + threadIdx.x;
-    if (w >= n_words) return;
-    const unsigned long long bit0 = w * 32ull;
-    unsigned long long i = bit0 / (unsigned)bits;
-    int sh = (int)(bit0 - i * (unsigned)bits);             // bits of token i that lie below this word
-    unsigned long long acc = i < n ? ((unsigned long long)ld_stream_u32(tok + i) >> sh) : 0ull;
-    int have = bits - sh;
-    for (i++; have < 32; i++, have += bits) acc |= (i < n ? (unsigned long long)ld_stream_u32(tok + i) : 0ull) << have;
-    out[w] = (uint32_t)acc;
 }
