@@ -90,6 +90,16 @@ const char *O200K_PAT =
     R"([^\r\n\p{L}\p{N}]?[\p{Lu}\p{Lt}\p{Lm}\p{Lo}\p{M}]+[\p{Ll}\p{Lm}\p{Lo}\p{M}]*(?i:'s|'t|'re|'ve|'m|'ll|'d)?|)"
     R"(\p{N}{1,3}| ?[^\s\p{L}\p{N}]+[\r\n/]*|\s*[\r\n]+|\s+(?!\S)|\s+)";
 
+// the PAT_* of pat_str, else -1 (and the B200BPE_EPATTERN message)
+int pattern_of(const char *pat_str) {
+    if (strcmp(pat_str, R50K_PAT) == 0) return PAT_R50K;
+    if (strcmp(pat_str, CL100K_PAT) == 0) return PAT_CL100K;
+    if (strcmp(pat_str, O200K_PAT) == 0) return PAT_O200K;
+    fail(B200BPE_EPATTERN, "unsupported pat_str: the GPU pre-tokeniser implements exactly the r50k/p50k, cl100k and "
+                           "o200k patterns of tiktoken_ext/openai_public.py (there is no CPU regex fallback)");
+    return -1;
+}
+
 // the calling thread's current device is restored when an ABI call returns (torch and friends keep per-thread state)
 struct DeviceGuard {
     int prev = -1;
@@ -114,6 +124,41 @@ struct DevBuf {
 
 struct PinnedBuf {
     void *p = nullptr; size_t cap = 0;
+};
+
+// What a pipeline run, a chunk, a device's worker or a whole call reports (the b200bpe_last_* getters).
+struct CallStats {
+    float ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};   // b200bpe_last_timings
+    uint32_t launches = 0;
+    uint32_t grown = 0, reruns = 0, token_passes = 0;
+    uint64_t cls[N_CLS] = {}; int lane_per_piece = 0;
+    uint64_t bytes_repairs = 0, unstable[5] = {}, memo[3] = {};
+
+    // the long pieces per class and the miss memo of a run whose output the call returns
+    void add_output(const Counters &c) {
+        for (int i = 0; i < N_CLS; i++) cls[i] += c.n_cls[i];
+        memo[0] += c.n_miss; memo[1] += c.n_owner; memo[2] += c.n_unplaced;
+    }
+    // everything but the timings and launches
+    void add_counts(const CallStats &o) {
+        grown |= o.grown; reruns += o.reruns;
+        for (int i = 0; i < N_CLS; i++) cls[i] += o.cls[i];
+        bytes_repairs += o.bytes_repairs;
+        for (int i = 0; i < 5; i++) unstable[i] += o.unstable[i];
+        for (int i = 0; i < 3; i++) memo[i] += o.memo[i];
+    }
+    // the next chunk of the same device: timings and launches add up
+    void add(const CallStats &o) {
+        for (int i = 0; i < 9; i++) ms[i] += o.ms[i];
+        launches += o.launches;
+        add_counts(o);
+    }
+    // another device's worker: each timing is the slowest device's, launches add up
+    void merge(const CallStats &o) {
+        for (int i = 0; i < 9; i++) ms[i] = std::max(ms[i], o.ms[i]);
+        launches += o.launches;
+        add_counts(o);
+    }
 };
 
 long env_long(const char *name, long dflt, long lo, long hi) {
@@ -205,8 +250,6 @@ struct Slot {
                                       // [14] bytes mode: start of the tail runs
     cudaEvent_t ev[N_EV];
     PinnedBuf stage;                // pinned staging for callers whose text is pageable memory
-    float last_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    uint32_t last_launches = 0;
     bool ok = false;
 
     cudaError_t init() {
@@ -269,7 +312,7 @@ struct UnstWs {
     DevBuf<uint32_t> res_tok, res_doc, grp; DevBuf<unsigned long long> res_off;
     UnstCounters *d_uc = nullptr, *h_uc = nullptr;   // h_uc pinned
     Counters *d_sctr = nullptr;              // the scans' total
-    void release() {
+    void release() {                         // the grow-only buffers; the counters stay
         it_lo.release(); it_cnt.release(); it_bytes.release(); it_doc.release(); item_base.release(); cbase.release();
         tbase.release(); part.release(); cinfo.release(); o_len.release(); s_len.release(); out_o.release(); out_s.release();
         nkeep.release(); slot.release(); keep.release(); kc.release(); o_off.release(); s_off.release(); tokoff_o.release();
@@ -313,6 +356,7 @@ struct PendingDeviceCall {             // the most recent b200bpe_encode_device*
     unsigned long long *d_tok_off = nullptr; unsigned long long *d_counts = nullptr;
     std::vector<uint8_t> sp_flags;        // the caller's special-token flags, copied (a re-run outlives the caller's array); empty: none
     cudaStream_t st = nullptr;
+    CallStats run;                        // the launches of its enqueue; the wait adds what it collects
 };
 
 struct b200bpe {
@@ -325,17 +369,27 @@ struct b200bpe {
     std::vector<uint32_t> tok_space;    // bit per id: all-space token (bytes mode; each device gets a copy on first use)
     std::vector<DevCtx *> devs;
     uint64_t table_bytes[4] = {0, 0, 0, 0};
-    float last_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-    uint32_t last_launches = 0;
-    // what the most recent encode call had to redo (b200bpe_last_reruns); reset by every encode entry point, before its
-    // argument checks and outside h->mu, hence atomic
-    std::atomic<uint32_t> last_grown{0}, last_reruns{0}, last_token_passes{0};
-    // long pieces per length class of the runs whose output the most recent encode call returned, and whether the
-    // lane-per-piece kernels merged them (b200bpe_last_piece_classes); reset with the re-run counters
-    std::atomic<uint64_t> last_cls[N_CLS] = {};
-    std::atomic<int> last_lane_per_piece{0};
-    std::atomic<uint64_t> last_bytes_repairs{0};   // documents the most recent bytes-mode call repaired (b200bpe_last_bytes_repairs)
-    std::atomic<uint64_t> last_unstable[5] = {};   // b200bpe_last_unstable
+    // what the most recent call reported; every encode entry point resets it before its argument checks and outside
+    // h->mu, hence a mutex of its own
+    std::mutex stats_mu; CallStats last;
+    void reset_stats() {                 // timings and launches stay those of the call before
+        std::lock_guard<std::mutex> lk(stats_mu);
+        CallStats z;
+        memcpy(z.ms, last.ms, sizeof(z.ms)); z.launches = last.launches;
+        last = z;
+    }
+    CallStats stats() { std::lock_guard<std::mutex> lk(stats_mu); return last; }
+    void publish(const CallStats &s) { std::lock_guard<std::mutex> lk(stats_mu); last = s; }
+    void publish_timings(const CallStats &s) {
+        std::lock_guard<std::mutex> lk(stats_mu);
+        memcpy(last.ms, s.ms, sizeof(s.ms)); last.launches = s.launches;
+    }
+    // a call that returns no output: what it redid and, with timings, the timings and launches of its runs
+    void publish_redo(const CallStats &s, bool timings = false) {
+        std::lock_guard<std::mutex> lk(stats_mu);
+        last.grown = s.grown; last.reruns = s.reruns; last.token_passes = s.token_passes;
+        if (timings) { memcpy(last.ms, s.ms, sizeof(s.ms)); last.launches = s.launches; }
+    }
     // completion search tables on the host, built by the first b200bpe_encode_with_unstable_batch call (then uploaded to
     // every device): mergeable ids in byte order, prefix sums of their lengths, all-space bits of the mergeable tokens,
     // per-id UTF-8 facts, and the byte_pair_encode of every token its own merges do not reach
@@ -344,21 +398,6 @@ struct b200bpe {
         std::vector<uint32_t> sorted, space, ur_idx, ur_off, ur_tok; std::vector<unsigned long long> lenpre;
         std::vector<uint8_t> u8info; uint32_t max_len = 0;
     } uh;
-    // missed pieces, those merged and those the memo could not place, of the runs whose output the most recent encode call
-    // returned (b200bpe_last_miss_memo)
-    std::atomic<uint64_t> last_memo[3] = {};
-    void reset_reruns() {
-        last_grown = 0; last_reruns = 0; last_token_passes = 0; last_bytes_repairs = 0;
-        for (auto &c : last_unstable) c = 0;
-        for (auto &c : last_memo) c = 0;
-        for (auto &c : last_cls) c = 0;
-        last_lane_per_piece = 0;
-    }
-    void set_piece_classes(const uint64_t *cls) {
-        for (int c = 0; c < N_CLS; c++) last_cls[c] = cls[c];
-        last_lane_per_piece = mid_group ? 0 : 1;
-    }
-    void set_miss_memo(const uint64_t *memo) { for (int i = 0; i < 3; i++) last_memo[i] = memo[i]; }
     size_t chunk_bytes = 64u << 20; bool chunk_forced = false;
     int copy_threads = 4;
     TaskPool *pool = nullptr;        // helper threads (created with the first host-path call)
@@ -415,6 +454,9 @@ static void devctx_destroy(DevCtx *D) {
     if (D->d_sp_arena) cudaFree(D->d_sp_arena);
     if (D->d_ut_arena) cudaFree(D->d_ut_arena);
     D->uw.release();
+    if (D->uw.d_uc) cudaFree(D->uw.d_uc);
+    if (D->uw.h_uc) cudaFreeHost(D->uw.h_uc);
+    if (D->uw.d_sctr) cudaFree(D->uw.d_sctr);
     delete D;
 }
 
@@ -475,13 +517,8 @@ extern "C" int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *to
                                     int n_dev, b200bpe_t **out) {
     if (!out || !pat_str || (n_tok && (!tok_bytes || !tok_off || !tok_rank)) || !devices || n_dev < 1)
         return fail(B200BPE_EINVAL, "null argument");
-    int pattern;
-    if (strcmp(pat_str, R50K_PAT) == 0) pattern = PAT_R50K;
-    else if (strcmp(pat_str, CL100K_PAT) == 0) pattern = PAT_CL100K;
-    else if (strcmp(pat_str, O200K_PAT) == 0) pattern = PAT_O200K;
-    else return fail(B200BPE_EPATTERN,
-                     "unsupported pat_str: the GPU pre-tokeniser implements exactly the r50k/p50k, cl100k and "
-                     "o200k patterns of tiktoken_ext/openai_public.py (there is no CPU regex fallback)");
+    const int pattern = pattern_of(pat_str);
+    if (pattern < 0) return B200BPE_EPATTERN;
     // the probe kernel tags a piece's token slot with the top two bits (kernels_encode.cuh PT_KIND), special ids included:
     // like the mergeable ranks (build_tables), every special id must stay below them
     for (uint32_t i = 0; i < n_sp; i++)
@@ -591,6 +628,7 @@ extern "C" int b200bpe_trim(b200bpe_t *h) {
             CUDA_TRY(cudaStreamSynchronize(D->slots[i].side2));
             D->slots[i].release_workspace();
         }
+        D->uw.release();
     }
     for (auto &b : h->pinned_pool) cudaFreeHost(b.p);
     h->pinned_pool.clear();
@@ -615,9 +653,41 @@ struct PipeArgs {
 
 static const unsigned long long MISS_CAP_MIN = 1u << 16, LONG_CAP_MIN = 1u << 20;
 
-// Enqueue the whole pipeline on args.st.  All pointers are device pointers on D->device; d_text must be 16-byte
-// aligned and readable up to n_bytes + 16.  No host synchronisation.
-static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
+// exclusive scan of n u32 counts into base[0..n] (base[n] = the sum, also in ctr->total_tokens), on st: three launches,
+// none when n == 0
+static cudaError_t enqueue_scan(const uint32_t *cnt, uint64_t n, unsigned long long *part, unsigned long long *base,
+                                Counters *ctr, cudaStream_t st) {
+    if (n == 0) {
+        cudaError_t e = cudaMemsetAsync(base, 0, 8, st);
+        return e != cudaSuccess ? e : cudaMemsetAsync(&ctr->total_tokens, 0, sizeof(ctr->total_tokens), st);
+    }
+    const long long nb = (long long)((n + SCAN_ITEMS - 1) / SCAN_ITEMS);
+    scan_partial_kernel<<<(unsigned)nb, 256, 0, st>>>(cnt, (long long)n, part);
+    scan_top_kernel<<<1, 1024, 0, st>>>(part, nb, ctr);
+    scan_final_kernel<<<(unsigned)nb, 256, 0, st>>>(cnt, (long long)n, part, base, ctr);
+    return cudaSuccess;
+}
+
+// The pre-tokeniser of `pattern` over n_words words of text: the fast rules, then the positions they left undecided
+// (two launches).  bytes: the haystack starts hbits may cut a document anywhere (kernels_bytes.cuh).
+static void enqueue_pretok(int pattern, bool bytes, int n_sm, cudaStream_t st, const uint8_t *text, long long n_bytes,
+                           const uint32_t *hbits, const UcTables &uc, uint32_t *pbits, uint32_t *psum, long long n_words,
+                           const uint32_t *ibits, uint32_t *slow, uint32_t scap, Counters *ctr) {
+    const unsigned grid = (unsigned)((n_words + 255) / 256);
+    auto launch = [&](auto pat) {
+        constexpr int P = decltype(pat)::value;
+        if (bytes) pretok_kernel<P, true><<<grid, 256, 0, st>>>(text, n_bytes, hbits, uc, pbits, psum, n_words, ibits, slow, scap, ctr);
+        else pretok_kernel<P><<<grid, 256, 0, st>>>(text, n_bytes, hbits, uc, pbits, psum, n_words, ibits, slow, scap, ctr);
+        pretok_slow_kernel<P><<<n_sm * 8, 256, 0, st>>>(text, n_bytes, hbits, uc, pbits, psum, slow, scap, ctr);
+    };
+    if (pattern == PAT_R50K) launch(std::integral_constant<int, PAT_R50K>());
+    else if (pattern == PAT_CL100K) launch(std::integral_constant<int, PAT_CL100K>());
+    else launch(std::integral_constant<int, PAT_O200K>());
+}
+
+// Enqueue the whole pipeline on args.st; run.launches = its kernel launches.  All pointers are device pointers on
+// D->device; d_text must be 16-byte aligned and readable up to n_bytes + 16.  No host synchronisation.
+static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a, CallStats &run) {
     const uint64_t n_bytes = a.n_bytes, n_docs = a.n_docs;
     cudaStream_t st = a.st;
     if (n_bytes >= (1ull << 32) - 4096) return fail(B200BPE_EINVAL, "batch too large for one call (>= 4 GiB)");
@@ -752,17 +822,8 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         unsigned grid = (unsigned)((n_words + 255) / 256);
         if (a.single_piece) single_piece_bits_kernel<<<grid, 256, 0, st>>>(S.w_pbits.p, S.w_psum.p, S.w_dbits.p, n_words);
         else {
-            const uint32_t scap = (uint32_t)std::min<size_t>(S.slow_cap, 0xFFFFFFF0u);
-#define B2_PRETOK(P)                                                                                                                   \
-    if (a.bytes) pretok_kernel<P, true><<<grid, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p,       \
-                                                             n_words, ibits, S.w_slow.p, scap, S.d_ctr);                              \
-    else pretok_kernel<P><<<grid, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, n_words, ibits,          \
-                                          S.w_slow.p, scap, S.d_ctr);                                                                  \
-    pretok_slow_kernel<P><<<D->n_sm * 8, 256, 0, st>>>(a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p, S.w_slow.p, scap, S.d_ctr)
-            if (h->pattern == PAT_R50K) { B2_PRETOK(PAT_R50K); }
-            else if (h->pattern == PAT_CL100K) { B2_PRETOK(PAT_CL100K); }
-            else { B2_PRETOK(PAT_O200K); }
-#undef B2_PRETOK
+            enqueue_pretok(h->pattern, a.bytes, D->n_sm, st, a.d_text, (long long)n_bytes, hbits, D->uc, S.w_pbits.p, S.w_psum.p,
+                           n_words, ibits, S.w_slow.p, (uint32_t)std::min<size_t>(S.slow_cap, 0xFFFFFFF0u), S.d_ctr);
             launches++;
         }
         launches++;
@@ -828,12 +889,7 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
         CUDA_TRY(cudaEventRecord(S.ev[7], st));
         CUDA_TRY(cudaStreamWaitEvent(st, S.ev[12], 0));          // join: the long pieces' tokens and counts are needed from here on
         CUDA_TRY(cudaStreamWaitEvent(st, S.ev[13], 0));
-        {
-            const long long nb = (n_tiles + SCAN_ITEMS - 1) / SCAN_ITEMS;
-            scan_partial_kernel<<<(unsigned)nb, 256, 0, st>>>(S.w_sub_count.p, n_tiles, S.w_scan_part.p);
-            scan_top_kernel<<<1, 1024, 0, st>>>(S.w_scan_part.p, nb, S.d_ctr);
-            scan_final_kernel<<<(unsigned)nb, 256, 0, st>>>(S.w_sub_count.p, n_tiles, S.w_scan_part.p, S.w_sub_base.p, S.d_ctr);
-        }
+        CUDA_TRY(enqueue_scan(S.w_sub_count.p, (uint64_t)n_tiles, S.w_scan_part.p, S.w_sub_base.p, S.d_ctr, st));
         const unsigned gather_grid = (unsigned)((n_tiles + GATHER_WARPS - 1) / GATHER_WARPS);
         const unsigned doc_grid = (unsigned)((n_docs + 1 + GATHER_WARPS - 1) / GATHER_WARPS);
         if (count_only) {            // only the sub-tiles that hold a document start, no token stores
@@ -869,26 +925,25 @@ static int enqueue_pipeline(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a) {
     if (a.bytes) CUDA_TRY(cudaMemcpyAsync(S.h_bytes, S.d_bytes, sizeof(BytesCounters), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(S.h_ctr, S.d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaEventRecord(S.ev[9], st));
-    S.last_launches = launches;
+    run.launches = launches;
     return B200BPE_OK;
 }
 
 static const int B200BPE_RETRY = 1;      // internal: capacities were grown, run the pipeline again
 
-// Wait for an enqueued pipeline, collect stage timings and device-side flags.  Returns B200BPE_RETRY when a
-// work-space that is sized from experience was too small for this batch (it has been grown to the exact need);
-// the B200BPE_GREW_* bits of the work-spaces that grew are then ORed into *grown.
-static int collect_pipeline(b200bpe *h, Slot &S, int *special_idx, uint64_t *special_pos, uint32_t *grown) {
-    (void)h;
+// Wait for an enqueued pipeline, collect stage timings (into run.ms) and device-side flags.  Returns B200BPE_RETRY
+// when a work-space that is sized from experience was too small for this batch (it has been grown to the exact need);
+// the B200BPE_GREW_* bits of the work-spaces that grew are then ORed into run.grown.
+static int collect_pipeline(Slot &S, CallStats &run, int *special_idx, uint64_t *special_pos) {
     CUDA_TRY(cudaEventSynchronize(S.ev[9]));
     CUDA_TRY(cudaGetLastError());
-    cudaEventElapsedTime(&S.last_ms[0], S.ev[0], S.ev[1]);
-    cudaEventElapsedTime(&S.last_ms[1], S.ev[1], S.ev[2]);
-    cudaEventElapsedTime(&S.last_ms[2], S.ev[11], S.ev[12]);     // long-piece kernels (side stream, overlapped with [3])
-    cudaEventElapsedTime(&S.last_ms[3], S.ev[3], S.ev[7]);
-    cudaEventElapsedTime(&S.last_ms[7], S.ev[7], S.ev[4]);
-    cudaEventElapsedTime(&S.last_ms[8], S.ev[3], S.ev[8]);
-    cudaEventElapsedTime(&S.last_ms[4], S.ev[0], S.ev[4]);
+    cudaEventElapsedTime(&run.ms[0], S.ev[0], S.ev[1]);
+    cudaEventElapsedTime(&run.ms[1], S.ev[1], S.ev[2]);
+    cudaEventElapsedTime(&run.ms[2], S.ev[11], S.ev[12]);     // long-piece kernels (side stream, overlapped with [3])
+    cudaEventElapsedTime(&run.ms[3], S.ev[3], S.ev[7]);
+    cudaEventElapsedTime(&run.ms[7], S.ev[7], S.ev[4]);
+    cudaEventElapsedTime(&run.ms[8], S.ev[3], S.ev[8]);
+    cudaEventElapsedTime(&run.ms[4], S.ev[0], S.ev[4]);
     const Counters &c = *S.h_ctr;
     if (c.err & ERR_DOCOFF)
         return fail(B200BPE_EINVAL, "document offsets must start at 0, be non-decreasing and end at n_bytes");
@@ -905,8 +960,8 @@ static int collect_pipeline(b200bpe *h, Slot &S, int *special_idx, uint64_t *spe
             S.miss_cap = std::max(S.miss_cap, (size_t)c.n_miss + (size_t)(c.n_miss / 8) + 4096);
             S.mres_cap = std::max(S.mres_cap, (size_t)c.miss_bytes + (size_t)(c.miss_bytes / 8) + 4096);
         }
-        *grown |= ((c.err & ERR_MISSCAP) ? B200BPE_GREW_MISS : 0u) | ((c.err & ERR_SLOWCAP) ? B200BPE_GREW_SLOW : 0u) |
-                  ((c.err & ERR_LONGCAP) ? B200BPE_GREW_LONG : 0u);
+        run.grown |= ((c.err & ERR_MISSCAP) ? B200BPE_GREW_MISS : 0u) | ((c.err & ERR_SLOWCAP) ? B200BPE_GREW_SLOW : 0u) |
+                     ((c.err & ERR_LONGCAP) ? B200BPE_GREW_LONG : 0u);
         return B200BPE_RETRY;
     }
     if (c.err & ERR_INTERNAL) return fail(B200BPE_ECUDA, "internal error: a merge kernel did not converge");
@@ -915,12 +970,26 @@ static int collect_pipeline(b200bpe *h, Slot &S, int *special_idx, uint64_t *spe
     return B200BPE_OK;
 }
 
-// what the miss memo did in the pipeline that last ran on S: missed pieces, pieces merged, pieces it could not place
-static void add_miss_memo(const Slot &S, uint64_t *memo) {
-    memo[0] += S.h_ctr->n_miss; memo[1] += S.h_ctr->n_owner; memo[2] += S.h_ctr->n_unplaced;
+// Collect the run enqueued on S; while a work-space was too small (it has been grown), enqueue() the same run again and
+// collect it, at most four more times.  run: the timings and launches of the last run, the re-runs, the work-spaces
+// grown and, on success, the long pieces per class and miss memo counters of the last run.
+static int collect_regrow(Slot &S, CallStats &run, int *special_idx, uint64_t *special_pos, const std::function<int()> &enqueue) {
+    int rc = collect_pipeline(S, run, special_idx, special_pos);
+    for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {
+        rc = enqueue();
+        if (!rc) { run.reruns++; rc = collect_pipeline(S, run, special_idx, special_pos); }
+    }
+    if (rc == B200BPE_RETRY) return fail(B200BPE_ECUDA, "work-space sizing did not converge");
+    if (!rc) run.add_output(*S.h_ctr);
+    return rc;
 }
 
-static int device_enqueue_locked(b200bpe *h, const PendingDeviceCall &c) {
+static bool any_flag(const b200bpe *h, const uint8_t *flags) {
+    if (flags) for (size_t i = 0; i < h->specials.size(); i++) if (flags[i]) return true;
+    return false;
+}
+
+static int device_enqueue_locked(b200bpe *h, const PendingDeviceCall &c, CallStats &run) {
     DevCtx *D = h->devs[0];
     Slot &S = D->slots[0];
     cudaStream_t st = c.st ? c.st : S.stream;
@@ -934,17 +1003,17 @@ static int device_enqueue_locked(b200bpe *h, const PendingDeviceCall &c) {
     a.d_text = txt; a.n_bytes = c.n_bytes; a.d_doc_off = c.d_doc_off; a.n_docs = c.n_docs; a.d_out = c.d_tokens;
     a.d_tok_off = c.d_tok_off; a.d_counts = c.d_counts; a.st = st;
     if (!c.sp_flags.empty()) a.sp_flags = c.sp_flags.data();
-    int rc = enqueue_pipeline(h, D, S, a);
+    int rc = enqueue_pipeline(h, D, S, a, run);
     if (rc || !a.sp_flags) return rc;
     special_sticky_kernel<<<1, 32, 0, st>>>(S.d_ctr, S.d_sticky);
-    S.last_launches++;
+    run.launches++;
     return B200BPE_OK;
 }
 
 extern "C" int b200bpe_encode_device_special_async(b200bpe_t *h, const uint8_t *d_text, uint64_t n_bytes,
                                                    const uint64_t *d_doc_off, uint64_t n_docs, const uint8_t *flags,
                                                    uint32_t *d_tokens, uint64_t *d_tok_off, uint64_t *d_counts, void *stream) {
-    if (h) h->reset_reruns();
+    if (h) h->reset_stats();
     if (!h || !d_doc_off || !d_tok_off || (n_bytes && !d_text)) return fail(B200BPE_EINVAL, "null argument");
     std::lock_guard<std::mutex> lk(h->mu);
     DeviceGuard guard;
@@ -954,10 +1023,8 @@ extern "C" int b200bpe_encode_device_special_async(b200bpe_t *h, const uint8_t *
     c.d_text = d_text; c.n_bytes = n_bytes; c.d_doc_off = (const unsigned long long *)d_doc_off; c.n_docs = n_docs;
     c.d_tokens = d_tokens; c.d_tok_off = (unsigned long long *)d_tok_off; c.d_counts = (unsigned long long *)d_counts;
     c.st = (cudaStream_t)stream;
-    bool any = false;
-    if (flags) for (size_t i = 0; i < h->specials.size(); i++) any |= flags[i] != 0;
-    if (any) c.sp_flags.assign(flags, flags + h->specials.size());
-    int rc = device_enqueue_locked(h, c);
+    if (any_flag(h, flags)) c.sp_flags.assign(flags, flags + h->specials.size());
+    int rc = device_enqueue_locked(h, c, c.run);
     if (rc) return rc;
     h->pending = std::move(c);
     return B200BPE_OK;
@@ -967,7 +1034,7 @@ extern "C" int b200bpe_encode_device_async(b200bpe_t *h, const uint8_t *d_text, 
                                            uint64_t n_docs, uint32_t *d_tokens, uint64_t *d_tok_off, uint64_t *d_counts,
                                            void *stream) {
     if (!d_tokens) {
-        if (h) h->reset_reruns();
+        if (h) h->reset_stats();
         return fail(B200BPE_EINVAL, "null argument");
     }
     return b200bpe_encode_device_special_async(h, d_text, n_bytes, d_doc_off, n_docs, nullptr, d_tokens, d_tok_off, d_counts,
@@ -976,7 +1043,7 @@ extern "C" int b200bpe_encode_device_async(b200bpe_t *h, const uint8_t *d_text, 
 
 extern "C" int b200bpe_device_wait_special(b200bpe_t *h, uint64_t *n_tokens, int32_t *special_index) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
-    h->reset_reruns();
+    h->reset_stats();
     std::lock_guard<std::mutex> lk(h->mu);
     if (!h->pending.active) return fail(B200BPE_EINVAL, "no device call in flight");
     DeviceGuard guard;
@@ -985,34 +1052,17 @@ extern "C" int b200bpe_device_wait_special(b200bpe_t *h, uint64_t *n_tokens, int
     Slot &S = D->slots[0];
     PendingDeviceCall c = h->pending;
     h->pending.active = false;
-    h->last_token_passes = 1;
     cudaStream_t st = c.st ? c.st : S.stream;
-    uint32_t grown = 0;                   // only what this wait grows: an earlier call of a queued series leaves sticky bits
+    CallStats &run = c.run;               // grown: only what this wait grows (an earlier call of a queued series leaves sticky bits)
+    run.token_passes = 1;
     int sidx = -1;
-    int rc = collect_pipeline(h, S, &sidx, nullptr, &grown);
-    h->last_grown = grown;
-    const uint64_t total = S.h_ctr->total_tokens;
+    const int rc = collect_regrow(S, run, &sidx, nullptr, [&] { return device_enqueue_locked(h, c, run); });
+    h->publish_redo(run, true);           // timings (no copies: [5] = [6] = 0) and launches even when the wait fails
     // error bits of the earlier calls of a queued series (the counters only describe the last one)
     unsigned int sticky[2] = {0, 0};      // error bits, 1 + the first disallowed special (special_sticky_kernel)
     CUDA_TRY(cudaMemcpyAsync(sticky, S.d_sticky, sizeof(sticky), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemsetAsync(S.d_sticky, 0, sizeof(sticky), st));
     CUDA_TRY(cudaStreamSynchronize(st));
-    uint64_t total2 = total;
-    bool reran = false;
-    for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {
-        rc = device_enqueue_locked(h, c);
-        if (rc) break;
-        h->last_reruns++;
-        rc = collect_pipeline(h, S, nullptr, nullptr, &grown);
-        h->last_grown = grown;
-        total2 = S.h_ctr->total_tokens;
-        CUDA_TRY(cudaMemsetAsync(S.d_sticky, 0, sizeof(sticky), st));
-        reran = true;
-    }
-    memcpy(h->last_ms, S.last_ms, sizeof(h->last_ms));
-    h->last_ms[5] = h->last_ms[6] = 0.f;
-    h->last_launches = S.last_launches;
-    if (rc == B200BPE_RETRY) return fail(B200BPE_ECUDA, "work-space sizing did not converge");
     // a disallowed special: the leftmost one of the earliest call of a queued series that has one.  sticky[1], not the
     // ERR_SPECIAL bit of sticky[0]: only device calls with flags set it, while finalize_kernel also ORs the error bits of
     // host-path pipelines on this slot into sticky[0] (a host call that failed on a disallowed special leaves it there)
@@ -1022,19 +1072,15 @@ extern "C" int b200bpe_device_wait_special(b200bpe_t *h, uint64_t *n_tokens, int
     }
     if (rc) return rc;
     if (c.queued > 1) {
-        if (reran || (sticky[0] & (ERR_LONGCAP | ERR_MISSCAP | ERR_SLOWCAP)))
+        if (run.reruns || (sticky[0] & (ERR_LONGCAP | ERR_MISSCAP | ERR_SLOWCAP)))
             return fail(B200BPE_ECAPACITY, "a work-space had to grow while several device calls were queued: only the last "
                                            "one was re-run, re-issue the others");
         if (sticky[0] & ERR_NOBYTE) return fail(B200BPE_ENOBYTE, "a piece needs a single-byte token that mergeable_ranks does not contain");
         if (sticky[0] & ERR_DOCOFF) return fail(B200BPE_EINVAL, "malformed document offsets in a queued device call");
     }
-    if (n_tokens) *n_tokens = total2;
-    uint64_t cls[N_CLS];                  // the last call of a queued series: the counters describe that one
-    for (int k = 0; k < N_CLS; k++) cls[k] = S.h_ctr->n_cls[k];
-    h->set_piece_classes(cls);
-    uint64_t memo[3] = {};
-    add_miss_memo(S, memo);
-    h->set_miss_memo(memo);
+    if (n_tokens) *n_tokens = S.h_ctr->total_tokens;
+    run.lane_per_piece = h->mid_group ? 0 : 1;
+    h->publish(run);                      // the last call of a queued series: the counters describe that one
     return B200BPE_OK;
 }
 
@@ -1048,43 +1094,21 @@ extern "C" int b200bpe_encode_device(b200bpe_t *h, const uint8_t *d_text, uint64
     return b200bpe_device_wait(h, n_tokens);
 }
 
-// exclusive scan of n u32 counts into base[0..n] (base[n] = the sum, also in ctr->total_tokens), on st
-static void enqueue_scan(const uint32_t *cnt, uint64_t n, unsigned long long *part, unsigned long long *base, Counters *ctr,
-                         cudaStream_t st) {
-    const long long nb = (long long)((n + SCAN_ITEMS - 1) / SCAN_ITEMS);
-    scan_partial_kernel<<<(unsigned)nb, 256, 0, st>>>(cnt, (long long)n, part);
-    scan_top_kernel<<<1, 1024, 0, st>>>(part, nb, ctr);
-    scan_final_kernel<<<(unsigned)nb, 256, 0, st>>>(cnt, (long long)n, part, base, ctr);
-}
-
 // A second run of the pipeline over text built on the device (bytes mode, completion search): enqueue, wait, and grow
-// and re-run while a work-space was too small; the long-piece classes and miss memo counters of the run are added.
-static int run_again(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a, uint64_t *cls, uint64_t *memo, uint32_t *grown,
-                     uint32_t *reruns) {
-    int rc = enqueue_pipeline(h, D, S, a);
-    if (!rc) rc = collect_pipeline(h, S, nullptr, nullptr, grown);
-    for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {   // a work-space grew: the same run again
-        rc = enqueue_pipeline(h, D, S, a);
-        if (!rc) { (*reruns)++; rc = collect_pipeline(h, S, nullptr, nullptr, grown); }
-    }
-    if (rc == B200BPE_RETRY) rc = fail(B200BPE_ECUDA, "work-space sizing did not converge");
-    if (rc) return rc;
-    for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
-    add_miss_memo(S, memo);
-    return B200BPE_OK;
+// and re-run while a work-space was too small.
+static int run_again(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a, CallStats &run) {
+    auto enqueue = [&] { return enqueue_pipeline(h, D, S, a, run); };
+    int rc = enqueue();
+    return rc ? rc : collect_regrow(S, run, nullptr, nullptr, enqueue);
 }
 
 // Bytes mode, a chunk whose run 1 (a1, counters in S.h_ctr and S.h_bytes) found documents that are not well-formed UTF-8: run 2 encodes
 // the unstable piece [u_d, end_d) of every such document as one piece, then the splice puts each document's run-1 tokens
 // minus the last kdrop[d] in front of its run-2 tokens.  The final tokens and offsets end up in S.w_out / S.w_tokoff and
 // *nt is their count.  Run 2 is sized from run 1's counters, which the host already waited for: that is the one extra
-// round trip of a damaged chunk.
-static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, uint64_t *nt, uint64_t *cls, uint64_t *memo,
-                           uint32_t *grown, uint32_t *reruns) {
+// round trip of a damaged chunk.  chunk: run 1's figures, to which the tail runs are added.
+static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, uint64_t *nt, CallStats &chunk) {
     const uint64_t n1 = S.h_ctr->total_tokens, drop = S.h_bytes->drop;
-    const float ms1[9] = {S.last_ms[0], S.last_ms[1], S.last_ms[2], S.last_ms[3], S.last_ms[4], S.last_ms[5], S.last_ms[6],
-                          S.last_ms[7], S.last_ms[8]};
-    const uint32_t launches1 = S.last_launches;
     const uint64_t nd = a1.n_docs, tail = S.h_bytes->tail;
     cudaStream_t st = a1.st;
     CUDA_TRY(S.w_b2doc.ensure((size_t)nd + 2)); CUDA_TRY(S.w_b2off.ensure((size_t)nd + 2)); CUDA_TRY(S.w_bbase.ensure((size_t)nd + 2));
@@ -1092,27 +1116,27 @@ static int bytes_tail_runs(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, u
     CUDA_TRY(S.w_btext.ensure((size_t)tail + 64)); CUDA_TRY(S.w_b2out.ensure((size_t)tail + 64));
     if (!S.d_bctr) CUDA_TRY(cudaMalloc((void **)&S.d_bctr, sizeof(Counters)));
     CUDA_TRY(cudaEventRecord(S.ev[14], st));
-    enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_b2doc.p, S.d_bctr, st);
+    CUDA_TRY(enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_b2doc.p, S.d_bctr, st));
     bytes_gather_kernel<<<(unsigned)((tail + 16 * 256 - 1) / (16 * 256)), 256, 0, st>>>(a1.d_text, nd, S.w_vup.p, S.w_b2doc.p, S.w_btext.p);
     PipeArgs a2;
     a2.d_text = S.w_btext.p; a2.n_bytes = tail; a2.d_doc_off = S.w_b2doc.p; a2.n_docs = nd;
     a2.d_out = S.w_b2out.p; a2.d_tok_off = S.w_b2off.p; a2.st = st; a2.single_piece = true;
-    int rc = run_again(h, D, S, a2, cls, memo, grown, reruns);
+    CallStats run2;
+    int rc = run_again(h, D, S, a2, run2);
     if (rc) return rc;
     float ms2 = 0; cudaEventElapsedTime(&ms2, S.ev[14], S.ev[4]);
-    const uint32_t launches2 = S.last_launches;
     *nt = n1 - drop + S.h_ctr->total_tokens;
     CUDA_TRY(S.w_bout.ensure((size_t)std::max<uint64_t>(*nt, a1.n_bytes) + 64));
     bytes_count_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, st>>>(S.w_tokoff.p, S.w_b2off.p, S.w_kdrop.p, nd, S.w_btail.p);
-    enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_bbase.p, S.d_bctr, st);
+    CUDA_TRY(enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_bbase.p, S.d_bctr, st));
     bytes_splice_kernel<<<(unsigned)std::min<uint64_t>(nd, (uint64_t)D->n_sm * 16), 256, 0, st>>>(
         S.w_out.p, S.w_tokoff.p, S.w_b2out.p, S.w_b2off.p, S.w_kdrop.p, S.w_bbase.p, nd, S.w_bout.p);
     CUDA_TRY(cudaGetLastError());
     std::swap(S.w_out, S.w_bout);
     std::swap(S.w_tokoff, S.w_bbase);
-    memcpy(S.last_ms, ms1, sizeof(ms1));
-    S.last_ms[4] += ms2;                  // device time of the chunk: run 1, then scan + gather + run 2
-    S.last_launches = launches1 + launches2 + 9;
+    chunk.ms[4] += ms2;                   // device time of the chunk: run 1, then scan + gather + run 2
+    chunk.launches += run2.launches + 9;
+    chunk.add_counts(run2);
     return B200BPE_OK;
 }
 
@@ -1235,29 +1259,19 @@ static cudaError_t grow_keep(DevBuf<Tp> &b, size_t used, size_t n, cudaStream_t 
     return cudaSuccess;
 }
 
-// exclusive scan of n u32 counts into base[0..n] (base[n] = the sum)
-static void uscan(UnstWs &W, const uint32_t *cnt, uint64_t n, unsigned long long *base, cudaStream_t st) {
-    if (n == 0) { cudaMemsetAsync(base, 0, 8, st); return; }
-    enqueue_scan(cnt, n, W.part.p, base, W.d_sctr, st);
-}
-
 struct UChunk {                  // one chunk's completions on the host
     std::vector<uint32_t> tok; std::vector<uint64_t> off, grp;   // off: n_comp + 1, grp: n_docs + 1
 };
 
 // Completion search of one chunk whose run 1 (a1, with the walk) has been collected: splices the stable tokens (run 1
 // minus each document's last L) into S.w_out / S.w_tokoff (*nt = their count), then searches, encodes, truncates and
-// deduplicates the candidates in rounds and brings the chunk's completions home.  stats: documents with unstable bytes,
-// candidates encoded, candidates through byte_pair_encode, rounds, completions.
-static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, UChunk &out, uint64_t *stats, uint64_t *nt,
-                           uint64_t *cls, uint64_t *memo, uint32_t *grown, uint32_t *reruns) {
+// deduplicates the candidates in rounds and brings the chunk's completions home.  chunk: run 1's figures; the runs of
+// the search add their counts (a deduplication retry counts as a re-run), not their timings or launches.
+static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, UChunk &out, uint64_t *nt, CallStats &chunk) {
     UnstWs &W = D->uw;
     const UnstTables &U = D->ut;
     const uint64_t nd = a1.n_docs;
     cudaStream_t st = a1.st;
-    const float ms1[9] = {S.last_ms[0], S.last_ms[1], S.last_ms[2], S.last_ms[3], S.last_ms[4], S.last_ms[5], S.last_ms[6],
-                          S.last_ms[7], S.last_ms[8]};
-    const uint32_t launches1 = S.last_launches;
     out.tok.clear(); out.off.assign(1, 0); out.grp.assign((size_t)nd + 1, 0);
     if (nd == 0) return B200BPE_OK;
     const uint64_t n1 = *nt;
@@ -1269,7 +1283,7 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
     if (!S.d_bctr) CUDA_TRY(cudaMalloc((void **)&S.d_bctr, sizeof(Counters)));
     CUDA_TRY(cudaMemsetAsync(W.zeros.p, 0, ((size_t)nd + 2) * 8, st));
     bytes_count_kernel<<<(unsigned)((nd + 255) / 256), 256, 0, st>>>(S.w_tokoff.p, W.zeros.p, S.w_kdrop.p, nd, S.w_btail.p);
-    enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_bbase.p, S.d_bctr, st);
+    CUDA_TRY(enqueue_scan(S.w_btail.p, nd, S.w_bpart.p, S.w_bbase.p, S.d_bctr, st));
     bytes_splice_kernel<<<(unsigned)std::min<uint64_t>(nd, (uint64_t)D->n_sm * 16), 256, 0, st>>>(
         S.w_out.p, S.w_tokoff.p, S.w_out.p, W.zeros.p, S.w_kdrop.p, S.w_bbase.p, nd, S.w_bout.p);
     std::swap(S.w_out, S.w_bout);
@@ -1278,7 +1292,7 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
     CUDA_TRY(W.item_base.ensure((size_t)nd + 2));
     CUDA_TRY(W.part.ensure((size_t)(nd / SCAN_ITEMS) + 4));
     CUDA_TRY(cudaMemsetAsync(W.d_uc, 0, sizeof(UnstCounters), st));
-    uscan(W, S.w_unit.p, nd, W.item_base.p, st);
+    CUDA_TRY(enqueue_scan(S.w_unit.p, nd, W.part.p, W.item_base.p, W.d_sctr, st));
     CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.item_base.p + nd, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[1], S.w_tokoff.p + nd, 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
@@ -1293,14 +1307,14 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
         unstable_search_kernel<<<(unsigned)((nd * 32 + 255) / 256), 256, 0, st>>>(U, a1.d_text, a1.d_doc_off, nd, S.w_ulen.p,
                                                                                  W.item_base.p, W.it_lo.p, W.it_cnt.p, W.it_bytes.p,
                                                                                  W.it_doc.p, W.d_uc);
-        uscan(W, W.it_cnt.p, n_items, W.cbase.p, st);
-        uscan(W, W.it_bytes.p, n_items, W.tbase.p, st);
+        CUDA_TRY(enqueue_scan(W.it_cnt.p, n_items, W.part.p, W.cbase.p, W.d_sctr, st));
+        CUDA_TRY(enqueue_scan(W.it_bytes.p, n_items, W.part.p, W.tbase.p, W.d_sctr, st));
         CUDA_TRY(cudaMemcpyAsync(W.h_uc, W.d_uc, sizeof(UnstCounters), cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.cbase.p + n_items, 8, cudaMemcpyDeviceToHost, st));
         CUDA_TRY(cudaStreamSynchronize(st));
         if (W.h_uc->err & UERR_BIG) return fail(B200BPE_EINVAL, "the completion candidates of one document need 4 GiB of text or more");
         n_cand = W.h_uc->tot[0];
-        stats[0] += W.h_uc->n_docs;
+        chunk.unstable[0] += W.h_uc->n_docs;
     }
     if (n_cand >= 0xFFFFFFF0ull) return fail(B200BPE_EINVAL, "too many completion candidates in one chunk (2^32)");
     UnstItems I;
@@ -1336,8 +1350,8 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
             CUDA_TRY(W.part.ensure((size_t)(2 * nr / SCAN_ITEMS) + 4));
             const unsigned grid = (unsigned)((nr + 255) / 256);
             unstable_meta_kernel<<<grid, 256, 0, st>>>(U, I, a1.d_text, c0, nr, W.cinfo.p, W.o_len.p, W.s_len.p, W.d_uc);
-            uscan(W, W.o_len.p, nr, W.o_off.p, st);
-            uscan(W, W.s_len.p, 2 * nr, W.s_off.p, st);
+            CUDA_TRY(enqueue_scan(W.o_len.p, nr, W.part.p, W.o_off.p, W.d_sctr, st));
+            CUDA_TRY(enqueue_scan(W.s_len.p, 2 * nr, W.part.p, W.s_off.p, W.d_sctr, st));
             CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.o_off.p + nr, 8, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[1], W.s_off.p + 2 * nr, 8, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaStreamSynchronize(st));
@@ -1350,8 +1364,10 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
                 PipeArgs a2;
                 a2.d_text = W.text_o.p; a2.n_bytes = ob; a2.d_doc_off = W.o_off.p; a2.n_docs = nr;
                 a2.d_out = W.out_o.p; a2.d_tok_off = W.tokoff_o.p; a2.st = st;
-                int rc = run_again(h, D, S, a2, cls, memo, grown, reruns);
+                CallStats run2;
+                int rc = run_again(h, D, S, a2, run2);
                 if (rc) return rc;
+                chunk.add_counts(run2);
             } else CUDA_TRY(cudaMemsetAsync(W.tokoff_o.p, 0, ((size_t)nr + 1) * 8, st));
             if (sb) {
                 CUDA_TRY(W.text_s.ensure((size_t)sb + 64)); CUDA_TRY(W.out_s.ensure((size_t)sb + 64));
@@ -1360,8 +1376,10 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
                 PipeArgs a3;
                 a3.d_text = W.text_s.p; a3.n_bytes = sb; a3.d_doc_off = W.s_off.p; a3.n_docs = 2 * nr;
                 a3.d_out = W.out_s.p; a3.d_tok_off = W.tokoff_s.p; a3.st = st; a3.single_piece = true;
-                int rc = run_again(h, D, S, a3, cls, memo, grown, reruns);
+                CallStats run2;
+                int rc = run_again(h, D, S, a3, run2);
                 if (rc) return rc;
+                chunk.add_counts(run2);
             } else CUDA_TRY(cudaMemsetAsync(W.tokoff_s.p, 0, (2 * (size_t)nr + 1) * 8, st));
             // truncate, deduplicate, append
             RunOut R{W.out_o.p, W.tokoff_o.p, W.out_s.p, W.tokoff_s.p};
@@ -1369,8 +1387,8 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
             CUDA_TRY(cudaMemsetAsync(S.d_bctr, 0, sizeof(Counters), st));
             unstable_insert_kernel<<<grid, 256, 0, st>>>(U, R, W.cinfo.p, S.w_ulen.p, c0, nr, seed, T, W.nkeep.p, W.slot.p, W.d_uc, S.d_bctr);
             unstable_verify_kernel<<<grid, 256, 0, st>>>(U, R, W.cinfo.p, c0, nr, T, res, W.nkeep.p, W.slot.p, W.keep.p, W.kc.p, W.d_uc);
-            uscan(W, W.keep.p, nr, W.rcb.p, st);
-            uscan(W, W.kc.p, nr, W.rtb.p, st);
+            CUDA_TRY(enqueue_scan(W.keep.p, nr, W.part.p, W.rcb.p, W.d_sctr, st));
+            CUDA_TRY(enqueue_scan(W.kc.p, nr, W.part.p, W.rtb.p, W.d_sctr, st));
             CUDA_TRY(cudaMemcpyAsync(W.h_uc, W.d_uc, sizeof(UnstCounters), cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[0], W.rcb.p + nr, 8, cudaMemcpyDeviceToHost, st));
             CUDA_TRY(cudaMemcpyAsync(&W.h_uc->tot[1], W.rtb.p + nr, 8, cudaMemcpyDeviceToHost, st));
@@ -1395,22 +1413,20 @@ static int unstable_search(b200bpe *h, DevCtx *D, Slot &S, const PipeArgs &a1, U
         if (!err) break;
         if (attempt >= 3) return fail(B200BPE_ECUDA, "completion deduplication did not converge");
         if (err & UERR_TABLE) W.tslots_min = slots * 4;   // else UERR_COLLIDE: the next attempt has another seed
-        (*reruns)++;
+        chunk.reruns++;
     }
     // ---- the chunk's completions: tokens, completion boundaries, per-document ranges
     CUDA_TRY(grow_keep(W.res_off, (size_t)(n_comp ? n_comp + 1 : 0), (size_t)n_comp + 2, st));
     W.h_uc->tot[2] = n_tok;
     CUDA_TRY(cudaMemcpyAsync(W.res_off.p + n_comp, &W.h_uc->tot[2], 8, cudaMemcpyHostToDevice, st));
-    uscan(W, W.grp.p, nd, W.grp_off.p, st);
+    CUDA_TRY(enqueue_scan(W.grp.p, nd, W.part.p, W.grp_off.p, W.d_sctr, st));
     out.tok.resize((size_t)n_tok); out.off.resize((size_t)n_comp + 1);
     if (n_tok) CUDA_TRY(cudaMemcpyAsync(out.tok.data(), W.res_tok.p, (size_t)n_tok * 4, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(out.off.data(), W.res_off.p, ((size_t)n_comp + 1) * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaMemcpyAsync(out.grp.data(), W.grp_off.p, ((size_t)nd + 1) * 8, cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     CUDA_TRY(cudaGetLastError());
-    stats[1] += enc; stats[2] += bpe; stats[3] += rounds; stats[4] += n_comp;
-    memcpy(S.last_ms, ms1, sizeof(ms1));
-    S.last_launches = launches1;
+    chunk.unstable[1] += enc; chunk.unstable[2] += bpe; chunk.unstable[3] += rounds; chunk.unstable[4] += n_comp;
     return B200BPE_OK;
 }
 
@@ -1429,13 +1445,8 @@ struct HostJob {
     std::atomic<int> error{0}; std::atomic<bool> overflow{false};
     std::string error_msg; std::mutex err_mu;
     int special_idx = -1; uint64_t special_pos = 0;
-    float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; std::mutex stat_mu;
-    uint32_t grown = 0, reruns = 0;               // B200BPE_GREW_* bits / pipeline re-runs of all workers (under stat_mu)
-    uint64_t cls[N_CLS] = {};                     // long pieces per length class of the chunks' final runs (under stat_mu)
-    uint64_t bytes_repairs = 0;                   // bytes mode: documents repaired (under stat_mu)
+    CallStats stats; std::mutex stat_mu;          // the workers that finished, merged (under stat_mu)
     std::vector<UChunk> uch;                      // completion search: chunk c's completions
-    uint64_t ustats[5] = {};                      // completion search: b200bpe_last_unstable (under stat_mu)
-    uint64_t memo[3] = {};                        // miss memo counters of the chunks' final runs (under stat_mu)
 
     void set_error(int rc) {
         std::lock_guard<std::mutex> lk(err_mu);
@@ -1513,40 +1524,34 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         return a;
     };
     size_t known = 0; uint64_t known_sum = 0;                    // prefix of the per-chunk token counts seen so far
-    float sum_ms[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0}; uint32_t launches = 0; float last_d2h = 0;
-    uint32_t grown = 0, reruns = 0;
-    uint64_t cls[N_CLS] = {}, repaired = 0, memo[3] = {}, ustats[5] = {};
+    std::vector<CallStats> chunk(mine.size());
+    CallStats worker;
     // finalise chunk k: wait for its kernels, then send its offsets + tokens home (async) at their final place
     auto drain = [&](size_t k) -> int {
         Slot &S = slot_of(k);
         const size_t c = mine[k];
         const uint64_t lo = J->cut[c], hi = J->cut[c + 1], nd = hi - lo;
+        CallStats &run = chunk[k];
         int sidx = -1; uint64_t spos = 0;
-        int rc = collect_pipeline(h, S, &sidx, &spos, &grown);
-        for (int attempt = 0; rc == B200BPE_RETRY && attempt < 4; attempt++) {   // a work-space grew: same chunk again
-            rc = enqueue_pipeline(h, D, S, args_of(k));
-            if (!rc) { reruns++; rc = collect_pipeline(h, S, &sidx, &spos, &grown); }
-        }
-        if (rc == B200BPE_RETRY) rc = fail(B200BPE_ECUDA, "work-space sizing did not converge");
+        int rc = collect_regrow(S, run, &sidx, &spos, [&] { return enqueue_pipeline(h, D, S, args_of(k), run); });
         if (rc == B200BPE_ESPECIAL) {
             std::lock_guard<std::mutex> lk(J->err_mu);
             const uint64_t gpos = spos + doc_off[lo];
             if (J->special_idx < 0 || gpos < J->special_pos) { J->special_idx = sidx; J->special_pos = gpos; }
         }
         if (rc) return rc;
-        float h2d = 0; cudaEventElapsedTime(&h2d, S.ev[5], S.ev[6]);
+        cudaEventElapsedTime(&run.ms[5], S.ev[5], S.ev[6]);
         uint64_t nt = S.h_ctr->total_tokens;
-        for (int i = 0; i < N_CLS; i++) cls[i] += S.h_ctr->n_cls[i];
-        add_miss_memo(S, memo);
         if (J->bytes && S.h_bytes->n_docs) {                     // documents that are not well-formed UTF-8: run 2 + splice
-            repaired += S.h_bytes->n_docs;
-            rc = bytes_tail_runs(h, D, S, args_of(k), &nt, cls, memo, &grown, &reruns);
+            run.bytes_repairs += S.h_bytes->n_docs;
+            rc = bytes_tail_runs(h, D, S, args_of(k), &nt, run);
             if (rc) return rc;
         }
         if (J->unstable) {                                       // stable tokens + the chunk's completions
-            rc = unstable_search(h, D, S, args_of(k), J->uch[c], ustats, &nt, cls, memo, &grown, &reruns);
+            rc = unstable_search(h, D, S, args_of(k), J->uch[c], &nt, run);
             if (rc) return rc;
         }
+        worker.add(run);
         J->count[c].store((long long)nt);
         while (known < c) {                                      // token base = counts of all earlier chunks (other devices)
             long long v = J->count[known].load();
@@ -1565,8 +1570,6 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         if (nt && !J->count_only)
             CUDA_TRY(cudaMemcpyAsync((uint32_t *)J->r->tok.p + token_base, S.w_out.p, nt * 4, cudaMemcpyDeviceToHost, S.stream));
         CUDA_TRY(cudaEventRecord(S.ev[6], S.stream));
-        for (int i = 0; i < 5; i++) sum_ms[i] += S.last_ms[i];
-        sum_ms[7] += S.last_ms[7]; sum_ms[8] += S.last_ms[8]; sum_ms[5] += h2d; launches += S.last_launches;
         return B200BPE_OK;
     };
     auto stop = [&]() { return J->error.load() != 0 || J->overflow.load(); };
@@ -1580,22 +1583,15 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     const size_t lag = J->unstable ? 0 : 1;
     for (size_t k = 0; k < mine.size() && !stop(); k++) {
         if (k + AHEAD < mine.size()) { rc = enqueue_h2d(k + AHEAD); if (rc) return bail(rc); }
-        rc = enqueue_pipeline(h, D, slot_of(k), args_of(k));
+        rc = enqueue_pipeline(h, D, slot_of(k), args_of(k), chunk[k]);
         if (rc) return bail(rc);
         if (k >= lag) { rc = drain(k - lag); if (rc) return bail(rc); }   // overlaps with chunk k's kernels (lag 1)
     }
     if (lag && !stop()) { rc = drain(mine.size() - 1); if (rc) return bail(rc); }
     bail(0);
-    if (!stop()) { Slot &S = slot_of(mine.size() - 1); cudaEventElapsedTime(&last_d2h, S.ev[5], S.ev[6]); }
+    if (!stop()) { Slot &S = slot_of(mine.size() - 1); cudaEventElapsedTime(&worker.ms[6], S.ev[5], S.ev[6]); }   // the last D2H
     std::lock_guard<std::mutex> lk(J->stat_mu);
-    for (int i = 0; i < 9; i++) J->sum_ms[i] = std::max(J->sum_ms[i], sum_ms[i]);       // per device; report the slowest
-    J->sum_ms[6] = std::max(J->sum_ms[6], last_d2h);
-    J->launches += launches;
-    J->grown |= grown; J->reruns += reruns;
-    for (int i = 0; i < N_CLS; i++) J->cls[i] += cls[i];
-    J->bytes_repairs += repaired;
-    for (int i = 0; i < 5; i++) J->ustats[i] += ustats[i];
-    for (int i = 0; i < 3; i++) J->memo[i] += memo[i];
+    J->stats.merge(worker);
 }
 
 // Chunk plan of the host path: document ranges [cut[c], cut[c+1]) of about `chunk` bytes each (a document larger than a
@@ -1645,6 +1641,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
         else pageable = (at.type == cudaMemoryTypeUnregistered);
     }
     // tokens <= bytes; bytes/2 covers everything but pathological text, which gets a second pass with the worst case
+    CallStats redo;                                               // grown, re-runs and token passes of all passes
     for (int pass = 0; pass < 2; pass++) {
         HostJob J;
         J.h = h; J.text = text; J.doc_off = doc_off; J.n_docs = n_docs; J.single_piece = single_piece; J.pageable = pageable;
@@ -1667,7 +1664,8 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
             for (int d = 0; d < workers; d++) th.emplace_back(host_worker, &J, d, (size_t)d, (size_t)workers);
             for (auto &t : th) t.join();
         }
-        h->last_grown |= J.grown; h->last_reruns += J.reruns; h->last_token_passes = (uint32_t)pass + 1;
+        redo.grown |= J.stats.grown; redo.reruns += J.stats.reruns; redo.token_passes = (uint32_t)pass + 1;
+        if (J.error.load() || J.overflow.load()) h->publish_redo(redo);
         if (J.error.load()) {
             g_last_error = J.error_msg;
             if (J.error.load() == B200BPE_ESPECIAL && special_idx) *special_idx = J.special_idx;
@@ -1676,11 +1674,10 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
         if (J.overflow.load()) { cleanup(0); continue; }
         uint64_t total = 0;
         for (auto &c : J.count) total += (uint64_t)std::max<long long>(0, c.load());
-        memcpy(h->last_ms, J.sum_ms, sizeof(J.sum_ms)); h->last_launches = J.launches;
         r->n_tokens = total;
-        h->set_piece_classes(J.cls);
-        h->last_bytes_repairs = J.bytes_repairs;
-        h->set_miss_memo(J.memo);
+        J.stats.grown = redo.grown; J.stats.reruns = redo.reruns; J.stats.token_passes = redo.token_passes;
+        J.stats.lane_per_piece = h->mid_group ? 0 : 1;
+        h->publish(J.stats);
         if (count_off) {
             memcpy(count_off, r->off.p, (size_t)(n_docs + 1) * 8);
             return cleanup(B200BPE_OK);
@@ -1700,7 +1697,6 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
             }
             r2->voff.push_back(r2->vtok.size());
             r2->n_tokens = r2->vtok.size(); r2->n_docs = r2->voff.size() - 1;
-            for (int i = 0; i < 5; i++) h->last_unstable[i] = J.ustats[i];
             h->live_results++;
             *completions = r2;
         }
@@ -1713,7 +1709,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
 
 extern "C" int b200bpe_encode_ordinary_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off,
                                              uint64_t n_docs, b200bpe_result_t **out) {
-    if (h) h->reset_reruns();
+    if (h) h->reset_stats();
     if (!h || !doc_off || !out) return fail(B200BPE_EINVAL, "null argument");
     if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
     std::lock_guard<std::mutex> lk(h->mu);
@@ -1726,7 +1722,7 @@ extern "C" int b200bpe_encode_ordinary_batch(b200bpe_t *h, const uint8_t *text, 
 // the device (kernels_bytes.cuh).
 extern "C" int b200bpe_encode_bytes_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                           b200bpe_result_t **out) {
-    if (h) h->reset_reruns();
+    if (h) h->reset_stats();
     if (!h || !doc_off || !out) return fail(B200BPE_EINVAL, "null argument");
     if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
     if (!h->decode_on_device)
@@ -1737,7 +1733,7 @@ extern "C" int b200bpe_encode_bytes_batch(b200bpe_t *h, const uint8_t *text, con
 }
 
 extern "C" int b200bpe_encode_single_piece(b200bpe_t *h, const uint8_t *piece, uint64_t len, b200bpe_result_t **out) {
-    if (h) h->reset_reruns();
+    if (h) h->reset_stats();
     if (!h || !out || (len && !piece)) return fail(B200BPE_EINVAL, "null argument");
     std::lock_guard<std::mutex> lk(h->mu);
     DeviceGuard guard;
@@ -1751,15 +1747,13 @@ extern "C" int b200bpe_encode_single_piece(b200bpe_t *h, const uint8_t *piece, u
 // emitted as their own ids.  flags[i]: 1 = allowed, 2 = disallowed, 0 = ordinary text.
 extern "C" int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                             const uint8_t *flags, b200bpe_result_t **out, int32_t *special_index) {
-    if (h) h->reset_reruns();
+    if (h) h->reset_stats();
     if (!h || !doc_off || !out) return fail(B200BPE_EINVAL, "null argument");
     if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
-    bool any = false;
-    if (flags) for (size_t i = 0; i < h->specials.size(); i++) any |= flags[i] != 0;
     std::lock_guard<std::mutex> lk(h->mu);
     DeviceGuard guard;
     int sidx = -1;
-    int rc = encode_host(h, text, doc_off, n_docs, false, any ? flags : nullptr, out, &sidx);
+    int rc = encode_host(h, text, doc_off, n_docs, false, any_flag(h, flags) ? flags : nullptr, out, &sidx);
     if (rc == B200BPE_ESPECIAL && special_index) *special_index = sidx;
     return rc;
 }
@@ -1768,15 +1762,13 @@ extern "C" int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, c
 // only the sub-tiles that hold a document start are gathered (without token stores); only the offsets come home.
 extern "C" int b200bpe_count_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                    const uint8_t *flags, uint64_t *tok_off, int32_t *special_index) {
-    if (h) h->reset_reruns();
+    if (h) h->reset_stats();
     if (!h || !doc_off || !tok_off) return fail(B200BPE_EINVAL, "null argument");
     if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
-    bool any = false;
-    if (flags) for (size_t i = 0; i < h->specials.size(); i++) any |= flags[i] != 0;
     std::lock_guard<std::mutex> lk(h->mu);
     DeviceGuard guard;
     int sidx = -1;
-    int rc = encode_host(h, text, doc_off, n_docs, false, any ? flags : nullptr, nullptr, &sidx, false, nullptr, tok_off);
+    int rc = encode_host(h, text, doc_off, n_docs, false, any_flag(h, flags) ? flags : nullptr, nullptr, &sidx, false, nullptr, tok_off);
     if (rc == B200BPE_ESPECIAL && special_index) *special_index = sidx;
     return rc;
 }
@@ -1784,7 +1776,7 @@ extern "C" int b200bpe_count_batch(b200bpe_t *h, const uint8_t *text, const uint
 extern "C" int b200bpe_encode_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                     const uint8_t *allowed, b200bpe_result_t **out) {
     if (!h) return fail(B200BPE_EINVAL, "null argument");
-    h->reset_reruns();
+    h->reset_stats();
     std::vector<uint8_t> flags(h->specials.size() + 1, 0);
     if (allowed) for (size_t i = 0; i < h->specials.size(); i++) flags[i] = allowed[i] ? 1 : 0;
     return b200bpe_encode_batch_special(h, text, doc_off, n_docs, allowed ? flags.data() : nullptr, out, nullptr);
@@ -1795,20 +1787,18 @@ extern "C" int b200bpe_encode_batch(b200bpe_t *h, const uint8_t *text, const uin
 extern "C" int b200bpe_encode_with_unstable_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                                   const uint8_t *flags, b200bpe_result_t **stable,
                                                   b200bpe_result_t **completions, int32_t *special_index) {
-    if (h) h->reset_reruns();
+    if (h) h->reset_stats();
     if (!h || !doc_off || !stable || !completions) return fail(B200BPE_EINVAL, "null argument");
     if (doc_off[n_docs] && !text) return fail(B200BPE_EINVAL, "null text");
     if (!h->decode_on_device)
         return fail(B200BPE_EINVAL, "the completion search reads token bytes from the device decode tables: every token id must be < 2^24");
-    bool any = false;
-    if (flags) for (size_t i = 0; i < h->specials.size(); i++) any |= flags[i] != 0;
     std::lock_guard<std::mutex> lk(h->mu);
     DeviceGuard guard;
     unstable_host_build(h);
     for (auto *D : h->devs) { int rc = unstable_upload(h, D); if (rc) return rc; }
     int sidx = -1;
     b200bpe_result *comp = nullptr;
-    int rc = encode_host(h, text, doc_off, n_docs, false, any ? flags : nullptr, stable, &sidx, false, &comp);
+    int rc = encode_host(h, text, doc_off, n_docs, false, any_flag(h, flags) ? flags : nullptr, stable, &sidx, false, &comp);
     if (rc == B200BPE_ESPECIAL && special_index) *special_index = sidx;
     if (!rc) *completions = comp;
     return rc;
@@ -1911,7 +1901,7 @@ extern "C" int b200bpe_decode_batch(b200bpe_t *h, const uint32_t *tokens, const 
         }
         ((uint64_t *)r->off.p)[n_docs] = k;
         r->n_tokens = k; rg.keep = true; h->live_results++;
-        memset(h->last_ms, 0, sizeof(h->last_ms)); h->last_launches = 0;
+        h->publish_timings(CallStats());
         *out = r;
         return B200BPE_OK;
     }
@@ -1929,13 +1919,8 @@ extern "C" int b200bpe_decode_batch(b200bpe_t *h, const uint32_t *tokens, const 
     if (n) CUDA_TRY(cudaMemcpyAsync(S.w_out.p, tokens, n * 4, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaMemcpyAsync(S.w_docoff.p, tok_off, (n_docs + 1) * 8, cudaMemcpyHostToDevice, st));
     CUDA_TRY(cudaEventRecord(S.ev[1], st));
-    const long long nn = (long long)n;
-    const long long nb = (nn + SCAN_ITEMS - 1) / SCAN_ITEMS;
     if (n) decode_len_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(S.w_out.p, n, D->d_tok_boff, h->n_ids, S.w_sub_count.p, S.d_ctr);
-    if (nb) scan_partial_kernel<<<(unsigned)nb, 256, 0, st>>>(S.w_sub_count.p, nn, S.w_scan_part.p);
-    scan_top_kernel<<<1, 1024, 0, st>>>(S.w_scan_part.p, nb, S.d_ctr);
-    if (nb) scan_final_kernel<<<(unsigned)nb, 256, 0, st>>>(S.w_sub_count.p, nn, S.w_scan_part.p, S.w_sub_base.p, S.d_ctr);
-    else CUDA_TRY(cudaMemsetAsync(S.w_sub_base.p, 0, 8, st));
+    CUDA_TRY(enqueue_scan(S.w_sub_count.p, n, S.w_scan_part.p, S.w_sub_base.p, S.d_ctr, st));
     CUDA_TRY(cudaMemcpyAsync(S.h_ctr, S.d_ctr, sizeof(Counters), cudaMemcpyDeviceToHost, st));
     CUDA_TRY(cudaStreamSynchronize(st));
     if (S.h_ctr->err & ERR_BADTOKEN) {
@@ -1960,11 +1945,12 @@ extern "C" int b200bpe_decode_batch(b200bpe_t *h, const uint32_t *tokens, const 
     CUDA_TRY(cudaEventRecord(S.ev[3], st));
     CUDA_TRY(cudaStreamSynchronize(st));
     CUDA_TRY(cudaGetLastError());
-    memset(h->last_ms, 0, sizeof(h->last_ms));
-    cudaEventElapsedTime(&h->last_ms[5], S.ev[0], S.ev[1]);
-    cudaEventElapsedTime(&h->last_ms[4], S.ev[1], S.ev[2]);
-    cudaEventElapsedTime(&h->last_ms[6], S.ev[2], S.ev[3]);
-    h->last_launches = 6;
+    CallStats run;
+    cudaEventElapsedTime(&run.ms[5], S.ev[0], S.ev[1]);
+    cudaEventElapsedTime(&run.ms[4], S.ev[1], S.ev[2]);
+    cudaEventElapsedTime(&run.ms[6], S.ev[2], S.ev[3]);
+    run.launches = 6;
+    h->publish_timings(run);
     rg.keep = true;
     h->live_results++;
     *out = r;
@@ -1973,43 +1959,48 @@ extern "C" int b200bpe_decode_batch(b200bpe_t *h, const uint32_t *tokens, const 
 
 extern "C" int b200bpe_last_timings(b200bpe_t *h, float *ms9, uint32_t *n_launches) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
-    if (ms9) memcpy(ms9, h->last_ms, sizeof(h->last_ms));
-    if (n_launches) *n_launches = h->last_launches;
+    const CallStats s = h->stats();
+    if (ms9) memcpy(ms9, s.ms, sizeof(s.ms));
+    if (n_launches) *n_launches = s.launches;
     return B200BPE_OK;
 }
 
 extern "C" int b200bpe_last_reruns(b200bpe_t *h, uint32_t *grown, uint32_t *reruns, uint32_t *token_passes) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
-    if (grown) *grown = h->last_grown.load();
-    if (reruns) *reruns = h->last_reruns.load();
-    if (token_passes) *token_passes = h->last_token_passes.load();
+    const CallStats s = h->stats();
+    if (grown) *grown = s.grown;
+    if (reruns) *reruns = s.reruns;
+    if (token_passes) *token_passes = s.token_passes;
     return B200BPE_OK;
 }
 
 extern "C" int b200bpe_last_piece_classes(b200bpe_t *h, uint64_t *counts8, int *lane_per_piece) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
-    if (counts8) for (int c = 0; c < N_CLS; c++) counts8[c] = h->last_cls[c].load();
-    if (lane_per_piece) *lane_per_piece = h->last_lane_per_piece.load();
+    const CallStats s = h->stats();
+    if (counts8) for (int c = 0; c < N_CLS; c++) counts8[c] = s.cls[c];
+    if (lane_per_piece) *lane_per_piece = s.lane_per_piece;
     return B200BPE_OK;
 }
 
 extern "C" int b200bpe_last_miss_memo(b200bpe_t *h, uint64_t *misses, uint64_t *merged, uint64_t *unplaced) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
-    if (misses) *misses = h->last_memo[0].load();
-    if (merged) *merged = h->last_memo[1].load();
-    if (unplaced) *unplaced = h->last_memo[2].load();
+    const CallStats s = h->stats();
+    if (misses) *misses = s.memo[0];
+    if (merged) *merged = s.memo[1];
+    if (unplaced) *unplaced = s.memo[2];
     return B200BPE_OK;
 }
 
 extern "C" int b200bpe_last_bytes_repairs(b200bpe_t *h, uint64_t *n_docs_repaired) {
     if (!h) return fail(B200BPE_EINVAL, "null handle");
-    if (n_docs_repaired) *n_docs_repaired = h->last_bytes_repairs.load();
+    if (n_docs_repaired) *n_docs_repaired = h->stats().bytes_repairs;
     return B200BPE_OK;
 }
 
 extern "C" int b200bpe_last_unstable(b200bpe_t *h, uint64_t *stats5) {
     if (!h || !stats5) return fail(B200BPE_EINVAL, "null argument");
-    for (int i = 0; i < 5; i++) stats5[i] = h->last_unstable[i].load();
+    const CallStats s = h->stats();
+    for (int i = 0; i < 5; i++) stats5[i] = s.unstable[i];
     return B200BPE_OK;
 }
 
@@ -2088,12 +2079,8 @@ extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, u
     if (stats8) for (int i = 0; i < 8; i++) stats8[i] = 0.0;
     if (n_merges_out) *n_merges_out = 0;
     if (!doc_off || !pat_str || !n_merges_out || (merges_cap && !merges_out)) return fail(B200BPE_EINVAL, "null argument");
-    int pattern;
-    if (strcmp(pat_str, R50K_PAT) == 0) pattern = PAT_R50K;
-    else if (strcmp(pat_str, CL100K_PAT) == 0) pattern = PAT_CL100K;
-    else if (strcmp(pat_str, O200K_PAT) == 0) pattern = PAT_O200K;
-    else return fail(B200BPE_EPATTERN, "unsupported pat_str: the GPU pre-tokeniser implements exactly the r50k/p50k, cl100k and "
-                                       "o200k patterns of tiktoken_ext/openai_public.py");
+    const int pattern = pattern_of(pat_str);
+    if (pattern < 0) return B200BPE_EPATTERN;
     if (vocab_size < 256) return fail(B200BPE_EINVAL, "vocab_size must be at least 256, so we can encode all bytes");
     if (doc_off[0] != 0) return fail(B200BPE_EINVAL, "document offsets must start at 0");
     const uint64_t N = doc_off[n_docs];
@@ -2166,15 +2153,8 @@ extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, u
         CUDA_TRY(cudaEventRecord(T.ev[0], s));
         mark_docs_kernel<<<(unsigned)((nd + 1 + 255) / 256), 256, 0, s>>>(T.doff.p, nd, n, T.dbits.p, T.sfd.p, nullptr, T.ctr);
         const unsigned grid = (unsigned)((n_words + 255) / 256);
-        const uint32_t scap = (uint32_t)std::min<uint64_t>(n + 64, 0xFFFFFFF0u);
-#define B2_TRAIN_PRETOK(P)                                                                                                  \
-    pretok_kernel<P><<<grid, 256, 0, s>>>(T.ct.p, (long long)n, T.dbits.p, uc, T.pbits.p, T.psum.p, n_words, nullptr,     \
-                                          T.slow.p, scap, T.ctr);                                                         \
-    pretok_slow_kernel<P><<<n_sm * 8, 256, 0, s>>>(T.ct.p, (long long)n, T.dbits.p, uc, T.pbits.p, T.psum.p, T.slow.p, scap, T.ctr)
-        if (pattern == PAT_R50K) { B2_TRAIN_PRETOK(PAT_R50K); }
-        else if (pattern == PAT_CL100K) { B2_TRAIN_PRETOK(PAT_CL100K); }
-        else { B2_TRAIN_PRETOK(PAT_O200K); }
-#undef B2_TRAIN_PRETOK
+        enqueue_pretok(pattern, false, n_sm, s, T.ct.p, (long long)n, T.dbits.p, uc, T.pbits.p, T.psum.p, n_words, nullptr,
+                       T.slow.p, (uint32_t)std::min<uint64_t>(n + 64, 0xFFFFFFF0u), T.ctr);
         CUDA_TRY(cudaEventRecord(T.ev[1], s));
         train_count_kernel<<<grid, 256, 0, s>>>(T.pbits.p, (long long)n, n_words, T.npieces.p);
         CUDA_TRY(cudaMemcpyAsync(T.h_ctr, T.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
@@ -2201,12 +2181,7 @@ extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, u
     CUDA_TRY(T.part.ensure((size_t)(n_tiles / SCAN_ITEMS) + 4));
     CUDA_TRY(cudaMemsetAsync(T.ctr, 0, sizeof(Counters), s));
     train_tile_count_kernel<<<(unsigned)((n_tiles + 255) / 256), 256, 0, s>>>(T.fbits.p, n_tiles, T.tcnt.p);
-    {
-        const long long nb = (n_tiles + SCAN_ITEMS - 1) / SCAN_ITEMS;
-        scan_partial_kernel<<<(unsigned)nb, 256, 0, s>>>(T.tcnt.p, n_tiles, T.part.p);
-        scan_top_kernel<<<1, 1024, 0, s>>>(T.part.p, nb, T.ctr);
-        scan_final_kernel<<<(unsigned)nb, 256, 0, s>>>(T.tcnt.p, n_tiles, T.part.p, T.tbase.p, T.ctr);
-    }
+    CUDA_TRY(enqueue_scan(T.tcnt.p, (uint64_t)n_tiles, T.part.p, T.tbase.p, T.ctr, s));
     CUDA_TRY(cudaMemcpyAsync(T.h_ctr, T.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(T.h_u64 + 1, T.wused.p, 8, cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
@@ -2216,16 +2191,9 @@ extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, u
     CUDA_TRY(T.dfirst.ensure(D + 2)); CUDA_TRY(T.dlen.ensure(D + 2)); CUDA_TRY(T.dcnt.ensure(D + 2)); CUDA_TRY(T.wl1.ensure(D + 2));
     CUDA_TRY(T.woff.ensure(D + 2));
     train_compact_kernel<<<n_sm * 8, 256, 0, s>>>(W, T.fbits.p, T.tbase.p, T.dfirst.p, T.dlen.p, T.dcnt.p, T.wl1.p, D, T.st);
-    {
-        const long long nb = ((long long)D + SCAN_ITEMS - 1) / SCAN_ITEMS;
-        CUDA_TRY(T.part.ensure((size_t)nb + 4));
-        CUDA_TRY(cudaMemsetAsync(T.ctr, 0, sizeof(Counters), s));
-        if (nb) {
-            scan_partial_kernel<<<(unsigned)nb, 256, 0, s>>>(T.wl1.p, (long long)D, T.part.p);
-            scan_top_kernel<<<1, 1024, 0, s>>>(T.part.p, nb, T.ctr);
-            scan_final_kernel<<<(unsigned)nb, 256, 0, s>>>(T.wl1.p, (long long)D, T.part.p, T.woff.p, T.ctr);
-        } else CUDA_TRY(cudaMemsetAsync(T.woff.p, 0, 8, s));
-    }
+    CUDA_TRY(T.part.ensure((size_t)((D + SCAN_ITEMS - 1) / SCAN_ITEMS) + 4));
+    CUDA_TRY(cudaMemsetAsync(T.ctr, 0, sizeof(Counters), s));
+    CUDA_TRY(enqueue_scan(T.wl1.p, D, T.part.p, T.woff.p, T.ctr, s));
     CUDA_TRY(cudaMemcpyAsync(T.h_ctr, T.ctr, sizeof(Counters), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaMemcpyAsync(T.h_st, T.st, sizeof(TrainState), cudaMemcpyDeviceToHost, s));
     CUDA_TRY(cudaStreamSynchronize(s));
