@@ -51,10 +51,13 @@ int b200bpe_create(const uint8_t *tok_bytes, const uint64_t *tok_off, const uint
                    const char *pat_str, int device, b200bpe_t **out);
 
 /* The same constructor for ONE engine spread over several GPUs of the box (SURVEY.md 8(b): `const int* devices,
- * int n_dev`): the tables are replicated on every listed device; the host-buffer entry points below cut a batch at
- * document boundaries into chunks that go round-robin over the devices (documents are independent haystacks,
- * src/lib.rs:360-373) and place every chunk's tokens at its final offset of one pinned result buffer -- the count
- * "gather" is a host prefix sum, no token payload crosses NVLink.  The device-resident entry points use devices[0]. */
+ * int n_dev`): the tables are replicated on every listed device; the host-buffer entry points below cut a batch into
+ * chunks that go round-robin over the devices and place every chunk's tokens at its final offset of one pinned result
+ * buffer -- the count "gather" is a host prefix sum, no token payload crosses NVLink.  Chunks end at document boundaries
+ * (documents are independent haystacks, src/lib.rs:360-373) and, in the encode and count entry points, also at seams
+ * inside documents larger than two chunks: a space between two ASCII letters, or a '\n' between a printable ASCII
+ * character and an ASCII letter or digit, where the split into pieces is provably that of the whole document, so
+ * outputs are unchanged (b200bpe_last_doc_seams).  The device-resident entry points use devices[0]. */
 int b200bpe_create_multi(const uint8_t *tok_bytes, const uint64_t *tok_off, const uint32_t *tok_rank,
                          uint32_t n_tok,
                          const uint8_t *sp_bytes, const uint64_t *sp_off, const uint32_t *sp_rank,
@@ -76,7 +79,10 @@ void b200bpe_destroy(b200bpe_t *h);
  * by Encoding.encode_ordinary_batch (tiktoken/core.py:164-176): ONE native call for the whole
  * batch.  text = concatenated UTF-8 of all documents, document d = [doc_off[d], doc_off[d+1]).
  * HOST buffers; the call copies them to the device, runs the kernels and brings back tokens
- * (uint32[n_tokens], documents concatenated) and offsets (uint64[n_docs+1]). */
+ * (uint32[n_tokens], documents concatenated) and offsets (uint64[n_docs+1]).  A document may have any length: one
+ * larger than two chunks is cut only at seams (see b200bpe_create_multi), which leaves the output unchanged; only a stretch
+ * of 4 GiB or more without a seam is refused (B200BPE_EINVAL).  The same holds for b200bpe_encode_batch,
+ * b200bpe_encode_batch_special and b200bpe_count_batch, whose seams also never fall inside a flagged special token. */
 int b200bpe_encode_ordinary_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off,
                                   uint64_t n_docs, b200bpe_result_t **out);
 
@@ -92,7 +98,8 @@ int b200bpe_encode_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_
  * encode_batch run first (tiktoken/core.py:120-124, :197-204, :431-438), both as ONE multi-pattern scan on the device.
  * flags[i] for special token i (index into the arrays given to b200bpe_create): 1 = allowed (cuts its document into
  * haystacks, emitted as its own id), 2 = disallowed (its presence anywhere fails the call with B200BPE_ESPECIAL and
- * *special_index = the leftmost offending special), 0 = ordinary text.  flags == NULL: no special handling. */
+ * *special_index = the leftmost offending special), 0 = ordinary text.  flags == NULL: no special handling.  Long
+ * documents as in b200bpe_encode_ordinary_batch: cut only at seams outside every flagged special, outputs unchanged. */
 int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                                  const uint8_t *flags, b200bpe_result_t **out, int32_t *special_index);
 
@@ -101,7 +108,8 @@ int b200bpe_encode_batch_special(b200bpe_t *h, const uint8_t *text, const uint64
  * d has tok_off[d+1] - tok_off[d] tokens.  flags as in b200bpe_encode_batch_special (NULL: ordinary); a disallowed
  * special fails with B200BPE_ESPECIAL and *special_index = the leftmost one.  No token leaves the device, and neither
  * the device output token buffer (4 bytes per input byte) nor a pinned token block is allocated; the long-piece and
- * special-token work-space (another 4 bytes per input byte) still is. */
+ * special-token work-space (another 4 bytes per input byte) still is.  Long documents as in
+ * b200bpe_encode_batch_special. */
 int b200bpe_count_batch(b200bpe_t *h, const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs,
                         const uint8_t *flags, uint64_t *tok_off, int32_t *special_index);
 
@@ -257,6 +265,11 @@ int b200bpe_last_unstable(b200bpe_t *h, uint64_t *stats5);
  * to 2^21.  After a queued device series the counts describe its last call.  Reset to zeros where b200bpe_last_reruns
  * is, and left at zeros by a call that fails. */
 int b200bpe_last_miss_memo(b200bpe_t *h, uint64_t *misses, uint64_t *merged, uint64_t *unplaced);
+
+/* How the most recent host-buffer encode or count call on this handle cut documents larger than a chunk: *seams =
+ * chunk boundaries placed inside documents, *docs_cut = documents with at least one of them.  Reset to zeros where
+ * b200bpe_last_reruns is, and left at zeros by a call that fails. */
+int b200bpe_last_doc_seams(b200bpe_t *h, uint64_t *seams, uint64_t *docs_cut);
 
 /* Sizes of the device tables (bytes) for reporting: [0] piece tables (narrow + wide), [1] pair table,
  * [2] long-token table + blob, [3] Unicode class tables. */

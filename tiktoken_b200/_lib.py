@@ -16,7 +16,7 @@ _CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "csrc")
 _SO = os.path.join(_CSRC, "libb200bpe.so")
 _SOURCES = ["b200bpe.cu", "dev_common.cuh", "kernels_pretok.cuh", "kernels_long.cuh", "kernels_mid.cuh", "kernels_pmerge.cuh", "kernels_encode.cuh",
             "kernels_special.cuh", "kernels_decode.cuh", "kernels_bytes.cuh", "kernels_unstable.cuh", "kernels_train.cuh", "utf8_check.cuh", "bpe_device.cuh", "bpe_tables.h", "pretok_rules.cuh",
-            "pretok_fast.cuh", "text_access.cuh", "unicode_classes.inc"]
+            "pretok_fast.cuh", "text_access.cuh", "unicode_classes.inc", "doc_seams.h"]
 
 OK, EINVAL, EPATTERN, EDUPRANK, ECUDA, ENOBYTE, EKEY, ESPECIAL, ECAPACITY, ENOPAIR = 0, -1, -2, -3, -4, -5, -6, -7, -8, -9
 
@@ -94,6 +94,8 @@ def lib() -> C.CDLL:
     L.b200bpe_last_unstable.argtypes = [vp, vp]
     L.b200bpe_last_miss_memo.restype = i32
     L.b200bpe_last_miss_memo.argtypes = [vp, C.POINTER(u64), C.POINTER(u64), C.POINTER(u64)]
+    L.b200bpe_last_doc_seams.restype = i32
+    L.b200bpe_last_doc_seams.argtypes = [vp, C.POINTER(u64), C.POINTER(u64)]
     L.b200bpe_encode_single_piece.restype = i32
     L.b200bpe_encode_single_piece.argtypes = [vp, vp, u64, C.POINTER(vp)]
     L.b200bpe_result_tokens.restype = vp
@@ -138,6 +140,7 @@ EXPORTS = [
     "b200bpe_last_piece_classes", "b200bpe_encode_bytes_batch", "b200bpe_last_bytes_repairs", "b200bpe_last_miss_memo",
     "b200bpe_encode_with_unstable_batch", "b200bpe_result_groups", "b200bpe_last_unstable", "b200bpe_bpe_train",
     "b200bpe_count_batch", "b200bpe_encode_device_special_async", "b200bpe_device_wait_special",
+    "b200bpe_last_doc_seams",
 ]
 
 GREW_MISS, GREW_SLOW, GREW_LONG = 1, 2, 4       # B200BPE_GREW_* (b200bpe_last_reruns)

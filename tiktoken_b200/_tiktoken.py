@@ -463,6 +463,14 @@ class CoreBPE:
         _lib.check(self._L.b200bpe_last_miss_memo(self._h, *(C.byref(x) for x in v)))
         return {"misses": int(v[0].value), "merged": int(v[1].value), "unplaced": int(v[2].value)}
 
+    def last_doc_seams(self) -> dict:
+        """How the most recent host-buffer encode or count call cut documents larger than a chunk: `seams` = chunk
+        boundaries placed inside documents (at word gaps or line starts, where the tokens do not change), `docs_cut` =
+        documents with at least one.  Zeros after a call that failed."""
+        seams, docs = C.c_uint64(0), C.c_uint64(0)
+        _lib.check(self._L.b200bpe_last_doc_seams(self._h, C.byref(seams), C.byref(docs)))
+        return {"seams": int(seams.value), "docs_cut": int(docs.value)}
+
     def trim(self) -> None:
         """Give the engine's grow-only device work-spaces and pooled pinned blocks back (tables stay)."""
         _lib.check(self._L.b200bpe_trim(self._h))

@@ -32,7 +32,8 @@
 // of the text, L2 probes of the rank tables and instruction issue.
 //
 // Host side: one DevCtx per CUDA device (tables replicated, three pipeline slots each); batches are cut at
-// document boundaries into chunks that go round-robin over the devices; H2D of chunk c+1, kernels of chunk c and
+// document boundaries, and documents larger than a chunk at seams (doc_seams.h), into chunks that go round-robin over
+// the devices; H2D of chunk c+1, kernels of chunk c and
 // D2H of chunk c-1 overlap on every device, and every chunk's tokens land at their final offset of ONE pinned
 // result buffer (the "gather" of SURVEY 8(e) is a host prefix sum over per-chunk counts).
 #include <cuda_runtime.h>
@@ -63,6 +64,7 @@
 #include "kernels_bytes.cuh"
 #include "kernels_unstable.cuh"
 #include "kernels_train.cuh"
+#include "doc_seams.h"
 #include "unicode_classes.inc"
 
 using namespace b2bpe;
@@ -133,6 +135,7 @@ struct CallStats {
     uint32_t grown = 0, reruns = 0, token_passes = 0;
     uint64_t cls[N_CLS] = {}; int lane_per_piece = 0;
     uint64_t bytes_repairs = 0, unstable[5] = {}, memo[3] = {};
+    uint64_t seams = 0, docs_cut = 0;    // chunks that start at a seam inside a document, documents with a seam
 
     // the long pieces per class and the miss memo of a run whose output the call returns
     void add_output(const Counters &c) {
@@ -146,6 +149,7 @@ struct CallStats {
         bytes_repairs += o.bytes_repairs;
         for (int i = 0; i < 5; i++) unstable[i] += o.unstable[i];
         for (int i = 0; i < 3; i++) memo[i] += o.memo[i];
+        seams += o.seams; docs_cut += o.docs_cut;
     }
     // the next chunk of the same device: timings and launches add up
     void add(const CallStats &o) {
@@ -1439,7 +1443,8 @@ struct HostJob {
     bool single_piece = false, pageable = false, bytes = false, unstable = false;
     bool count_only = false;                      // token offsets only: no device token buffer, no token download
     const uint8_t *sp_flags = nullptr;
-    std::vector<uint64_t> cut;                    // chunk c = documents [cut[c], cut[c+1])
+    const ChunkPlan *plan = nullptr;              // chunk c = parts [cut[c], cut[c+1]) (doc_seams.h)
+    const uint64_t *part_off = nullptr;           // the parts' byte offsets: plan->part_off, or doc_off when nothing was cut
     std::vector<std::atomic<long long>> count;    // tokens of chunk c, -1 until its kernels are done
     b200bpe_result *r = nullptr; size_t tok_cap = 0;
     std::atomic<int> error{0}; std::atomic<bool> overflow{false};
@@ -1458,7 +1463,8 @@ struct HostJob {
 static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     b200bpe *h = J->h;
     DevCtx *D = h->devs[dev_index];
-    const size_t n_chunks = J->cut.size() - 1;
+    const std::vector<uint64_t> &cut = J->plan->cut;
+    const size_t n_chunks = cut.size() - 1;
     std::vector<size_t> mine;
     for (size_t c = first; c < n_chunks; c += step) mine.push_back(c);
     auto bail = [&](int rc) {
@@ -1468,7 +1474,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     };
     if (mine.empty()) return;
     if (cudaSetDevice(D->device) != cudaSuccess) { fail(B200BPE_ECUDA, "cudaSetDevice failed"); return bail(B200BPE_ECUDA); }
-    const uint64_t *doc_off = J->doc_off;
+    const uint64_t *part_off = J->part_off;
     auto slot_of = [&](size_t k) -> Slot & { return D->slots[k % DevCtx::N_SLOTS]; };
 
     // Upload of chunk k into its slot.  Pinned caller memory: on the slot's own stream, i.e. behind the download of the
@@ -1478,7 +1484,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     auto enqueue_h2d = [&](size_t k) -> int {
         Slot &S = slot_of(k);
         const size_t c = mine[k];
-        const uint64_t lo = J->cut[c], hi = J->cut[c + 1], b0 = doc_off[lo], nb = doc_off[hi] - b0, nd = hi - lo;
+        const uint64_t lo = cut[c], hi = cut[c + 1], b0 = part_off[lo], nb = part_off[hi] - b0, nd = hi - lo;
         const bool staged = J->pageable && nb;
         cudaStream_t us = staged ? S.up : S.stream;
         if (!staged || S.w_text.cap < (size_t)nb + 64 || S.w_docoff.cap < (size_t)nd + 2 || S.w_tokoff.cap < (size_t)nd + 2 ||
@@ -1507,7 +1513,7 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
                 CUDA_TRY(cudaMemcpyAsync(S.w_text.p + g0, stg + g0, len, cudaMemcpyHostToDevice, us));
             }
         } else if (nb) CUDA_TRY(cudaMemcpyAsync(S.w_text.p, src, nb, cudaMemcpyHostToDevice, us));
-        CUDA_TRY(cudaMemcpyAsync(S.w_docoff.p, doc_off + lo, (nd + 1) * 8, cudaMemcpyHostToDevice, us));
+        CUDA_TRY(cudaMemcpyAsync(S.w_docoff.p, part_off + lo, (nd + 1) * 8, cudaMemcpyHostToDevice, us));
         if (b0) add_offset_kernel<<<(unsigned)((nd + 1 + 255) / 256), 256, 0, us>>>(S.w_docoff.p, nd + 1, -(long long)b0);
         CUDA_TRY(cudaEventRecord(S.ev[6], us));
         if (staged) CUDA_TRY(cudaStreamWaitEvent(S.stream, S.ev[6], 0));     // the slot's pipeline starts when its text has arrived
@@ -1516,9 +1522,9 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     auto args_of = [&](size_t k) {
         Slot &S = slot_of(k);
         const size_t c = mine[k];
-        const uint64_t lo = J->cut[c], hi = J->cut[c + 1];
+        const uint64_t lo = cut[c], hi = cut[c + 1];
         PipeArgs a;
-        a.d_text = S.w_text.p; a.n_bytes = doc_off[hi] - doc_off[lo]; a.d_doc_off = S.w_docoff.p; a.n_docs = hi - lo;
+        a.d_text = S.w_text.p; a.n_bytes = part_off[hi] - part_off[lo]; a.d_doc_off = S.w_docoff.p; a.n_docs = hi - lo;
         a.d_out = J->count_only ? nullptr : S.w_out.p; a.d_tok_off = S.w_tokoff.p; a.st = S.stream; a.single_piece = J->single_piece; a.sp_flags = J->sp_flags;
         a.bytes = J->bytes; a.unstable = J->unstable;
         return a;
@@ -1530,13 +1536,13 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     auto drain = [&](size_t k) -> int {
         Slot &S = slot_of(k);
         const size_t c = mine[k];
-        const uint64_t lo = J->cut[c], hi = J->cut[c + 1], nd = hi - lo;
+        const uint64_t lo = cut[c], hi = cut[c + 1], nd = hi - lo;
         CallStats &run = chunk[k];
         int sidx = -1; uint64_t spos = 0;
         int rc = collect_regrow(S, run, &sidx, &spos, [&] { return enqueue_pipeline(h, D, S, args_of(k), run); });
         if (rc == B200BPE_ESPECIAL) {
             std::lock_guard<std::mutex> lk(J->err_mu);
-            const uint64_t gpos = spos + doc_off[lo];
+            const uint64_t gpos = spos + part_off[lo];
             if (J->special_idx < 0 || gpos < J->special_pos) { J->special_idx = sidx; J->special_pos = gpos; }
         }
         if (rc) return rc;
@@ -1551,6 +1557,8 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
             rc = unstable_search(h, D, S, args_of(k), J->uch[c], &nt, run);
             if (rc) return rc;
         }
+        const uint8_t head = J->plan->head[c];
+        run.seams = head ? 1 : 0; run.docs_cut = head == 2 ? 1 : 0;
         worker.add(run);
         J->count[c].store((long long)nt);
         while (known < c) {                                      // token base = counts of all earlier chunks (other devices)
@@ -1566,7 +1574,12 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
         if (!J->count_only && token_base + nt > J->tok_cap) { J->overflow.store(true); return B200BPE_OK; }
         if (token_base) add_offset_kernel<<<(unsigned)((nd + 1 + 255) / 256), 256, 0, S.stream>>>(S.w_tokoff.p, nd + 1, (long long)token_base);
         CUDA_TRY(cudaEventRecord(S.ev[5], S.stream));
-        CUDA_TRY(cudaMemcpyAsync((uint64_t *)J->r->off.p + lo, S.w_tokoff.p, (nd + 1) * 8, cudaMemcpyDeviceToHost, S.stream));
+        // the offsets of the documents that start in the chunk (after its first part when that continues a document cut
+        // at a seam), and the last chunk's end: every entry of the result is written once, and no seam is
+        const uint64_t d0 = J->plan->first_doc[c], d1 = J->plan->first_doc[c + 1] + (c + 1 == n_chunks ? 1 : 0);
+        if (d1 > d0)
+            CUDA_TRY(cudaMemcpyAsync((uint64_t *)J->r->off.p + d0, S.w_tokoff.p + (head ? 1 : 0), (d1 - d0) * 8,
+                                     cudaMemcpyDeviceToHost, S.stream));
         if (nt && !J->count_only)
             CUDA_TRY(cudaMemcpyAsync((uint32_t *)J->r->tok.p + token_base, S.w_out.p, nt * 4, cudaMemcpyDeviceToHost, S.stream));
         CUDA_TRY(cudaEventRecord(S.ev[6], S.stream));
@@ -1594,28 +1607,17 @@ static void host_worker(HostJob *J, int dev_index, size_t first, size_t step) {
     J->stats.merge(worker);
 }
 
-// Chunk plan of the host path: document ranges [cut[c], cut[c+1]) of about `chunk` bytes each (a document larger than a
-// chunk is a chunk of its own); one chunk when the batch is at most 1.5 chunks or in single-piece mode.
-static int chunk_plan(const uint64_t *doc_off, uint64_t n_docs, size_t chunk, bool single_piece, std::vector<uint64_t> &cut) {
-    const uint64_t n_bytes = doc_off[n_docs];
-    cut.assign(1, 0);
-    if (!single_piece && n_bytes > chunk + chunk / 2) {
-        uint64_t lo = 0;
-        while (lo < n_docs) {
-            const uint64_t want = doc_off[lo] + chunk;
-            uint64_t hi = (uint64_t)(std::upper_bound(doc_off + lo, doc_off + n_docs + 1, want) - doc_off);   // first off > want
-            if (hi > 0) hi--;                                    // last doc boundary <= want
-            if (hi <= lo) hi = lo + 1;                           // a single document larger than a chunk
-            if (hi > n_docs) hi = n_docs;
-            cut.push_back(hi); lo = hi;
-        }
-    } else cut.push_back(n_docs);
-    for (size_t c = 0; c + 1 < cut.size(); c++) {
-        const uint64_t cb = doc_off[cut[c + 1]] - doc_off[cut[c]];
-        if (doc_off[cut[c + 1]] < doc_off[cut[c]] || cb >= (1ull << 32) - 4096)
-            return fail(B200BPE_EINVAL, cb >= (1ull << 32) - 4096 ? "a single document of >= 4 GiB is not supported"
-                                                                  : "document offsets must be non-decreasing");
-    }
+// Chunk plan of the host path (doc_seams.h plan_chunks), with its errors as B200BPE_EINVAL
+static int chunk_plan(const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, size_t chunk, PlanMode mode,
+                      const SeamSpecials &sp, ChunkPlan &plan) {
+    const int rc = plan_chunks(text, doc_off, n_docs, chunk, mode, sp, plan);
+    if (rc == PLAN_UNORDERED) return fail(B200BPE_EINVAL, "document offsets must be non-decreasing");
+    if (rc == PLAN_TOO_LARGE)
+        return fail(B200BPE_EINVAL, mode == PLAN_SEAMS
+                                        ? "a document has a stretch of >= 4 GiB without a seam (a word gap or line start "
+                                          "where it may be cut): not supported"
+                                        : "a single document of >= 4 GiB is not supported in bytes mode, the completion "
+                                          "search, single-piece mode or training");
     return B200BPE_OK;
 }
 
@@ -1628,12 +1630,17 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
     const int n_dev = (int)h->devs.size();
     if (!h->pool) h->pool = new TaskPool();
     h->pool->ensure(h->copy_threads);
-    // ---- chunk plan: document ranges [lo, hi) ------------------------------------------------
+    // ---- chunk plan: ranges of parts, i.e. of documents and, for documents larger than a chunk, of their pieces between
+    // seams.  Bytes mode and the completion search read each document from its first ill-formed byte or its last piece
+    // to its end, so their documents are not cut.
     size_t chunk = h->chunk_bytes;
     if (!h->chunk_forced && n_dev > 1) chunk = std::min<size_t>(64u << 20, std::max<size_t>(8u << 20, (size_t)(n_bytes / (4 * (uint64_t)n_dev))));
-    std::vector<uint64_t> cut;
-    if (int rc = chunk_plan(doc_off, n_docs, chunk, single_piece, cut)) return rc;
-    const size_t n_chunks = cut.size() - 1;
+    const PlanMode mode = single_piece ? PLAN_WHOLE : (bytes || completions) ? PLAN_DOCS : PLAN_SEAMS;
+    SeamSpecials sp;
+    sp.str = h->specials.data(); sp.n = h->specials.size(); sp.flags = sp_flags;
+    ChunkPlan plan;
+    if (int rc = chunk_plan(text, doc_off, n_docs, chunk, mode, sp, plan)) return rc;
+    const size_t n_chunks = plan.cut.size() - 1;
     bool pageable = false;
     if (n_bytes) {
         cudaPointerAttributes at;
@@ -1645,7 +1652,7 @@ static int encode_host(b200bpe *h, const uint8_t *text, const uint64_t *doc_off,
     for (int pass = 0; pass < 2; pass++) {
         HostJob J;
         J.h = h; J.text = text; J.doc_off = doc_off; J.n_docs = n_docs; J.single_piece = single_piece; J.pageable = pageable;
-        J.sp_flags = sp_flags; J.cut = cut; J.bytes = bytes; J.unstable = completions != nullptr; J.count_only = count_off != nullptr;
+        J.sp_flags = sp_flags; J.plan = &plan; J.part_off = plan.part_off.empty() ? doc_off : plan.part_off.data(); J.bytes = bytes; J.unstable = completions != nullptr; J.count_only = count_off != nullptr;
         if (J.unstable) J.uch.resize(n_chunks);
         J.count = std::vector<std::atomic<long long>>(n_chunks);
         for (auto &c : J.count) c.store(-1);
@@ -2004,6 +2011,14 @@ extern "C" int b200bpe_last_unstable(b200bpe_t *h, uint64_t *stats5) {
     return B200BPE_OK;
 }
 
+extern "C" int b200bpe_last_doc_seams(b200bpe_t *h, uint64_t *seams, uint64_t *docs_cut) {
+    if (!h) return fail(B200BPE_EINVAL, "null handle");
+    const CallStats s = h->stats();
+    if (seams) *seams = s.seams;
+    if (docs_cut) *docs_cut = s.docs_cut;
+    return B200BPE_OK;
+}
+
 extern "C" int b200bpe_table_bytes(b200bpe_t *h, uint64_t *bytes4) {
     if (!h || !bytes4) return fail(B200BPE_EINVAL, "null argument");
     memcpy(bytes4, h->table_bytes, sizeof(h->table_bytes));
@@ -2087,8 +2102,9 @@ extern "C" int b200bpe_bpe_train(const uint8_t *text, const uint64_t *doc_off, u
     if (N && !text) return fail(B200BPE_EINVAL, "null text");
     size_t chunk = env_chunk_bytes();
     if (!chunk) chunk = 64u << 20;
-    std::vector<uint64_t> cut;
-    if (int rc = chunk_plan(doc_off, n_docs, chunk, false, cut)) return rc;
+    ChunkPlan plan;                                         // the words of a document are counted whole: no seams
+    if (int rc = chunk_plan(text, doc_off, n_docs, chunk, PLAN_DOCS, SeamSpecials(), plan)) return rc;
+    const std::vector<uint64_t> &cut = plan.cut;
     const uint32_t target = vocab_size;
     if (target == 256) return B200BPE_OK;                  // the 256 single bytes, no merge
     if (merges_cap > 0xFFFFFFF0ull) merges_cap = 0xFFFFFFF0ull;

@@ -171,6 +171,35 @@ extern "C" int hc_piece_starts_fast_cut(int pattern, const uint8_t *text, int64_
     return piece_starts_fast<true>(pattern, text, n, doc_off, n_docs, is_start, stats2);
 }
 
+// the host path's seam rule and chunk plan (doc_seams.h), as b200bpe.cu runs them
+#include "doc_seams.h"
+
+extern "C" int hc_is_seam(const uint8_t *text, uint64_t doc_lo, uint64_t doc_hi, uint64_t p) {
+    return is_seam(text, doc_lo, doc_hi, p) ? 1 : 0;
+}
+// specials: sp_n strings, string i = sp_bytes[sp_off[i] .. sp_off[i+1]); flags NULL: no special handling.  Returns the
+// number of chunks n (or -1 - PlanError); when n <= cap: bounds[0..n] = the chunks' byte bounds, first_doc[0..n] and
+// head[0..n-1] as in ChunkPlan; stats2 = {seams, docs_cut}.
+extern "C" int64_t hc_plan_chunks(const uint8_t *text, const uint64_t *doc_off, uint64_t n_docs, uint64_t chunk, int mode,
+                                  const uint8_t *sp_bytes, const uint64_t *sp_off, uint64_t sp_n, const uint8_t *flags,
+                                  uint64_t cap, uint64_t *bounds, uint64_t *first_doc, uint8_t *head, uint64_t *stats2) {
+    std::vector<std::string> specials;
+    for (uint64_t i = 0; i < sp_n; i++) specials.emplace_back((const char *)sp_bytes + sp_off[i], (size_t)(sp_off[i + 1] - sp_off[i]));
+    SeamSpecials sp;
+    sp.str = specials.data(); sp.n = specials.size(); sp.flags = flags;
+    ChunkPlan P;
+    const int rc = plan_chunks(text, doc_off, n_docs, chunk, (PlanMode)mode, sp, P);
+    if (rc) return -1 - rc;
+    const uint64_t n = P.cut.size() - 1;
+    const uint64_t *po = P.part_off.empty() ? doc_off : P.part_off.data();
+    if (n <= cap) {
+        for (uint64_t c = 0; c <= n; c++) { bounds[c] = po[P.cut[c]]; first_doc[c] = P.first_doc[c]; }
+        for (uint64_t c = 0; c < n; c++) head[c] = P.head[c];
+    }
+    stats2[0] = P.seams; stats2[1] = P.docs_cut;
+    return (int64_t)n;
+}
+
 // the UTF-8 classifier of the bytes mode (utf8_check.cuh): valid_up_to of every document (its length when well-formed),
 // from the first mark of each document, the way utf8_check_kernel reduces them
 #include "utf8_check.cuh"
